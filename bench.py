@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- images/s of the ViT-VQGAN fwd+bwd hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- images/s of the ViT-VQGAN fwd+bwd hot path (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
         --master-port 29500 bench.py --gpus 8 --steps 5 --warmup 3
     python bench.py --impl reference --steps 3 --warmup 1      # the CPU arm (reference modules / oracle port)
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs out/   # also write the last timed step's results as .npy
 
 One "step" = x -> ViTEncoder -> pre_quant -> VectorQuantizer -> post_quant -> ViTDecoder ->
 loss = mean((rec-x)^2) + qloss -> backward, fp32 parameters, no optimizer step (SURVEY.md
@@ -26,7 +27,7 @@ sys.path.insert(0, ROOT)
 
 METRIC = "images/sec (256x256) ViT-VQGAN fwd+bwd"
 UNIT = "images/s"
-FP32_FMA_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12     # 148 SMs x 128 FMA lanes x 2 FLOP x 1.965 GHz = 74.5
+FP32_FMA_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12      # H100 SXM: 132 SMs x 128 FMA lanes x 2 FLOP x 1.98 GHz = 66.9
 
 
 def load_peaks():
@@ -36,7 +37,8 @@ def load_peaks():
             p = json.load(f)
         return dict(hbm_gbs=p["hbm_gbs"], bf16_tflops=p["bf16_tflops"], bf16_tflops_sustained=p["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0,
+                source="NVIDIA H100 SXM data sheet (dense, 700 W board), not measured")
 
 
 class ClockSampler:
@@ -77,7 +79,7 @@ class ClockSampler:
 # ------------------------------------------------------------------------------------------------
 def reference_modules():
     """the reference's layers.py / quantizers.py, vendored unmodified into oracle/_ref by oracle/build_ref.py
-    (git-ignored; they travel to the GPU box with the snapshot).  None if absent."""
+    (git-ignored).  None if absent."""
     ref_dir = os.path.join(ROOT, "oracle", "_ref", "enhancing_ref")
     if not (os.path.exists(os.path.join(ref_dir, "layers.py")) and os.path.exists(os.path.join(ref_dir, "quantizers.py"))):
         return None
@@ -192,7 +194,7 @@ def run_reference(args):
 
 
 def gpu_eager_baseline(cfg_name, dev, batches=(64, 48, 32, 16, 8)):
-    """the reference modules .cuda() eagerly on this B200 (cuBLAS / cuDNN / ATen): the honest 'reference on this
+    """the reference modules .cuda() eagerly on this GPU (cuBLAS / cuDNN / ATen): the honest 'reference on this
     box' bar (SURVEY.md section 8d), at the largest batch that fits, with TF32 matmuls off and on"""
     import torch
     out = {}
@@ -241,7 +243,7 @@ def vq_block(dev, peaks):
     E = torch.randn(K, D, generator=g).to(dev)
     z_rand = torch.randn(M, D, generator=g).to(dev)
     z_clu = (E[torch.randint(0, 45, (M,), generator=g).to(dev)] + 0.01 * torch.randn(M, D, generator=g).to(dev)).contiguous()
-    flush = torch.empty(160 * 2 ** 20 // 4, device=dev)           # > 126 MB L2: written between timed launches
+    flush = torch.empty(160 * 2 ** 20 // 4, device=dev)           # > 50 MB L2: written between timed launches
 
     def timed(fn, iters=5):
         for _ in range(2):
@@ -269,8 +271,27 @@ def vq_block(dev, peaks):
         res[name]["live_codes"] = int(idx[:, 0].unique().numel())
     res["note"] = ("forward time includes vq_prep (codebook normalise + transpose) and the loss reduction; the lookup is FP32-FMA "
                    "bound (1986 FLOP/B), so GB/s is a few % of HBM by construction and the kernel is graded on frac_of_fp32_fma_peak "
-                   f"(peak {FP32_FMA_PEAK_TFLOPS:.1f} TFLOP/s = 148 SM x 128 lanes x 2 x 1.965 GHz)")
+                   f"(peak {FP32_FMA_PEAK_TFLOPS:.1f} TFLOP/s = 132 SM x 128 lanes x 2 x 1.98 GHz)")
     return res
+
+
+DUMP_SAMPLE = 32768      # elements kept of each larger gradient: ~25 MB in all at the base config
+
+
+def dump_outputs(out_dir, model, loss):
+    """what one timed step hands its caller: the loss, the reconstruction (first two images) and every parameter's
+    gradient -- whole up to DUMP_SAMPLE elements, otherwise a fixed sample (seeded by the tensor's position)"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(float(loss.detach()), dtype=np.float64))
+    np.save(os.path.join(out_dir, "rec.npy"), model.last_rec[:2].float().cpu().numpy())
+    for i, (name, p) in enumerate(model.named_parameters()):
+        if p.grad is None:
+            continue
+        g = p.grad.detach().float().reshape(-1).cpu().numpy()
+        if g.size > DUMP_SAMPLE:
+            g = g[np.sort(np.random.default_rng(i).choice(g.size, DUMP_SAMPLE, replace=False))]
+        np.save(os.path.join(out_dir, f"grad.{name}.npy"), g)
 
 
 def main():
@@ -286,9 +307,13 @@ def main():
     ap.add_argument("--ref-batch", type=int, default=4, help="images per CPU step for --impl reference / cpu_baseline")
     ap.add_argument("--ddp", action="store_true", help="torch DistributedDataParallel (overlapped buckets) instead of one flat all-reduce")
     ap.add_argument("--no-fuse-pos", action="store_true", help="keep post_quant and the decoder's positional add separate")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last timed step's loss, reconstruction sample and gradient samples to DIR/*.npy")
     ap.add_argument("--extras", default="vq,secondary,eager,cpu",
                     help="comma list of the 1-GPU extra blocks to measure after the timed regions: vq, secondary, eager, cpu ('' = none)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -303,7 +328,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device: the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs a CUDA device: the CUDA path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -330,6 +355,8 @@ def main():
         def forward(self, x):
             quant, qloss, _ = self.quantizer(self.pre_quant(self.encoder(x)))
             rec = self.decoder(self.post_quant(quant))
+            if args.dump_outputs:
+                self.last_rec = rec.detach()
             return ((rec - x) ** 2).mean() + qloss
 
     def barrier():
@@ -403,7 +430,7 @@ def main():
     barrier()
     ev0.record()
     for _ in range(args.steps):
-        step(dev_imgs)
+        loss_last = step(dev_imgs)
     ev1.record()
     barrier()
     launches = etb.ops.launch_count() - launches0
@@ -416,6 +443,8 @@ def main():
     n_gemm = len(gemm_events)
     comm_ms = sum(s.elapsed_time(e) for s, e in comm_events) / max(1, args.steps)
     comm_events.clear()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, loss_last)
 
     # ---- end-to-end timed region: pinned host images in (prefetched on a copy stream), loss out, every step ----
     copy_stream = torch.cuda.Stream(device=dev)
@@ -457,7 +486,7 @@ def main():
         flops_step = 3.0 * flops_per_image(cfg) * B
         achieved = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
         peak = peaks["bf16_tflops_sustained"]
-        kern = {"fp16": "gemm_tc_kernel<KIND=f16> (tcgen05 kind::f16, fp32 accumulate)", "tf32": "gemm_tc_kernel<KIND=tf32> (tcgen05 kind::tf32)",
+        kern = {"fp16": "gemm_tc_kernel<KIND=f16> (mma.sync m16n8k16 f16, fp32 accumulate)", "tf32": "gemm_tc_kernel<KIND=tf32> (mma.sync m16n8k8 tf32)",
                 "parity": "gemm_tc_kernel<KIND=tf32>, 3 passes (3xTF32)"}[precision]
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": warm,
@@ -466,8 +495,8 @@ def main():
                       "tf32": "tf32", "parity": "3xtf32 (fp32-grade)"}[precision], "data": "synthetic",
             "config": {"workload": f"imagenet_vitvq_{args.config}.yaml shapes (ViT-VQGAN-{args.config}), synthetic 256x256x3, "
                                    f"fwd+bwd, batch {B}/GPU", "global_batch": world * B, "per_gpu_batch": B,
-                       "parallelism": f"dp{world}", "l2_hygiene": "inputs_exceed_l2 (activations >> 126 MB per step)",
-                       "gemm_cta_group": args.cta_group, "precision": precision, "post_quant_pos_fused": not args.no_fuse_pos,
+                       "parallelism": f"dp{world}", "l2_hygiene": "inputs_exceed_l2 (activations >> 50 MB per step)",
+                       "gemm_tile": "128 x 128 (128 x 64 for outputs <= 64 columns and for 3xTF32), one CTA per tile", "precision": precision, "post_quant_pos_fused": not args.no_fuse_pos,
                        "grad_reduce": ("torch DDP buckets (overlapped)" if args.ddp else "one flat NCCL all-reduce after backward") if world > 1 else "none"},
             "model_tflops_per_gpu": flops_step / (ms_total / args.steps / 1e3) / 1e12,
             "clocks": clocks,
@@ -477,11 +506,8 @@ def main():
             "gpu_launches": int(launches),
             "roofline": {"bound": "tensor", "kernel": kern, "achieved": achieved, "peak": peak,
                          "unit": "TFLOP/s", "frac": achieved / peak,
-                         "traffic": 7.544e8 if (args.config == "base" and B == 128 and precision == "fp16") else None,
-                         "traffic_note": "dram read+write bytes of one to_qkv launch (M=131072 N=2304 K=768, fp16 in/out) from profiles/r02_ncu_gemm_f16.txt "
-                                         "(ncu --set full); algorithmic bytes of that launch: 8.09e8 (A 201 MB + B 3.5 MB + C 604 MB); tensor pipe 86 % "
-                                         "active there, 90 % on the K=3072 net.2 launch",
-                         "peak_source": peaks["source"] + ": cuBLAS bf16 sustained (kind::f16 issues at the bf16 rate; kind::tf32 at half of it)",
+                         "traffic": None,
+                         "peak_source": peaks["source"] + " (f16 mma issues at the bf16 rate; tf32 at half of it)",
                          "launches_timed": n_gemm, "share_of_step": gemm_ms / ms_total,
                          "algorithmic_gemm_tflop_per_step": 3.0 * gemm_flops_per_image(cfg) * B / 1e12,
                          "f16_gemms": {"achieved": f16_flops / (f16_ms / 1e3) / 1e12 if f16_ms > 0 else None,

@@ -1,4 +1,4 @@
-"""B200-native ViT-VQGAN hot path (see DESIGN.md).  Import as ``enhancing_transformers_b200``.
+"""CUDA-native (H100, sm_90a) ViT-VQGAN hot path (see DESIGN.md).  Import as ``enhancing_transformers_b200``.
 
     import enhancing_transformers_b200 as etb
     etb.patch()          # rebind Encoder / Decoder / VectorQuantizer inside the reference's vitvqgan.py

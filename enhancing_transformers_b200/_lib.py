@@ -66,7 +66,7 @@ EXPORTS = tuple(_SIGNATURES)
 
 
 def build(verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into libb200vq.so (in-tree, next to this file)."""
+    """Compile csrc/*.cu for sm_90a into libb200vq.so (in-tree, next to this file)."""
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -32,10 +32,10 @@ int current_device() {
 int num_sms() {
   static PerDevice cache;
   const int dev = current_device();
-  if (dev < 0 || dev >= kMaxDevices) return 148;
+  if (dev < 0 || dev >= kMaxDevices) return 132;
   if (!cache.done[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache.value[dev] = n;
     cache.done[dev] = true;
   }
@@ -116,7 +116,7 @@ extern "C" {
 
 int b200vq_version(void) { return B200VQ_VERSION; }
 const char* b200vq_last_error(void) { return g_err; }
-const char* b200vq_arch(void) { return "sm_100a"; }
+const char* b200vq_arch(void) { return "sm_90a"; }
 long long b200vq_launch_count(void) { return g_launches.load(); }
 
 int b200vq_set_sm_limit(int n) { g_sm_limit.store(n < 0 ? 0 : n); return 0; }

@@ -2,8 +2,8 @@
 // q k^T * scale -> softmax -> . v) and the row-wise helper of its backward.
 //
 // The reference materialises and saves a [B, heads, N, N] fp32 probability tensor per layer
-// (6.4 GB at B=128, base).  Here the scores live in tensor memory only (attention_tc.cu:
-// tcgen05 / TMEM flash-style forward and backward); backward recomputes them from the saved
+// (6.4 GB at B=128, base).  Here the scores live in registers only (attention_exact.cu:
+// mma.sync flash-style forward and backward); backward recomputes them from the saved
 // log-sum-exp and needs delta = rowsum(dO * O), computed below.
 #include "common.cuh"
 
@@ -97,7 +97,7 @@ int attention_backward(const float* qkv, const void* out, int out_half, const fl
 // Stage-2 attention (reference enhancing/modules/stage2/layers.py:76-89): causal mask whose first cond_len tokens (the
 // condition prefix) see each other fully -- query q attends to key k iff k <= max(q, cond_len - 1).  Same packed qkv layout
 // as the stage-1 core (the reference's (T, B*nh, hs) views are that layout transposed).  exact != 0: 3xTF32 mma.sync kernels
-// (precision="parity"); otherwise the tcgen05 kind::tf32 kernels with the mask folded into their padding logic.
+// (precision="parity"); otherwise the single-pass tf32 kernels with the same mask.
 int attention_causal_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale, int cond_len,
                              int exact, int round_out, cudaStream_t stream) {
   B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");

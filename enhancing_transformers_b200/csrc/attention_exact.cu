@@ -1,34 +1,45 @@
-// "Exact" attention core for the parity mode: the same flash-style algorithm as attention_tc.cu
-// (reference enhancing/modules/stage1/layers.py:124-130 and its autograd), but every tensor-core product is the
-// error-compensated 3xTF32 form  a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi  (hi = the 10-bit-mantissa truncation the
-// tensor core would apply anyway, lo = x - hi, exact in fp32), issued as three mma.sync m16n8k8 instructions with the
-// operands split in registers.  fp32-grade results (~2^-21 relative) at a fraction of the tcgen05 kernels' speed:
-// it exists so that `precision="parity"` can be checked against the reference with margin, not to be fast.
+// Flash-style attention core on mma.sync, tf32 m16n8k8 or f16 m16n8k16 (reference enhancing/modules/stage1/layers.py:124-130 and its
+// autograd): the scores live in registers only, backward recomputes them from the saved log-sum-exp.
+//   PASSES == 1: one tf32 product per MMA; the softmax probabilities and dS are rounded to nearest tf32 before they
+//                re-enter the tensor core.  Serves the tf32 data path (q/k/v already tf32-rounded by the GEMM that wrote
+//                them).
+//   IN16:        the fp16 data path: fp16 q/k/v/dO staged as fp16, mma.sync m16n8k16 .f16 with ldmatrix fragments,
+//                probabilities and dS packed to fp16 pairs in registers (struct Ops below).
+//   PASSES == 3: the error-compensated 3xTF32 form  a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi  (hi = the
+//                10-bit-mantissa truncation the tensor core applies anyway, lo = x - hi, exact in fp32), split in
+//                registers: fp32-grade results (~2^-21 relative) for `precision="parity"`.
+// IN16 / OUT16 select fp16 storage of the inputs (q/k/v, dO) and of the outputs (O, dq/dk/dv).
 // Backward is split in two kernels so that no atomics are needed: one CTA per key tile (dK, dV) and one per
-// query tile (dQ); scores are recomputed from the saved log-sum-exp.
+// query tile (dQ).
 #include "common.cuh"
+
+#include <type_traits>
 
 namespace b200 {
 
 constexpr float kLog2e = 1.4426950408889634f;
 
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 constexpr uint32_t kTf32Mask = 0xFFFFE000u;
 __device__ __forceinline__ uint32_t tf32_hi(uint32_t x) { return x & kTf32Mask; }
 __device__ __forceinline__ uint32_t tf32_lo(uint32_t x) { return __float_as_uint(__uint_as_float(x) - __uint_as_float(x & kTf32Mask)) & kTf32Mask; }
-// c += a . b with both operands given as raw fp32 bit patterns: small terms first
-__device__ __forceinline__ void mma_3xtf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  const uint32_t ah[4] = {tf32_hi(a[0]), tf32_hi(a[1]), tf32_hi(a[2]), tf32_hi(a[3])};
-  const uint32_t al[4] = {tf32_lo(a[0]), tf32_lo(a[1]), tf32_lo(a[2]), tf32_lo(a[3])};
-  mma_tf32(c, al, tf32_hi(b0), tf32_hi(b1));
-  mma_tf32(c, ah, tf32_lo(b0), tf32_lo(b1));
-  mma_tf32(c, ah, tf32_hi(b0), tf32_hi(b1));
+// c += a . b with both operands given as raw fp32 bit patterns (3 passes: small terms first)
+template <int PASSES>
+__device__ __forceinline__ void mma_x(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (PASSES == 1) {
+    mma_tf32(c, a, b0, b1);
+  } else {
+    const uint32_t ah[4] = {tf32_hi(a[0]), tf32_hi(a[1]), tf32_hi(a[2]), tf32_hi(a[3])};
+    const uint32_t al[4] = {tf32_lo(a[0]), tf32_lo(a[1]), tf32_lo(a[2]), tf32_lo(a[3])};
+    mma_tf32(c, al, tf32_hi(b0), tf32_hi(b1));
+    mma_tf32(c, ah, tf32_lo(b0), tf32_lo(b1));
+    mma_tf32(c, ah, tf32_hi(b0), tf32_hi(b1));
+  }
 }
+// one element as fp32 bits, from fp32 or fp16 storage
+__device__ __forceinline__ uint32_t ldbits(const float* p) { return __float_as_uint(*p); }
+__device__ __forceinline__ uint32_t ldbits(const __half* p) { return __float_as_uint(__half2float(*p)); }
+// row pitch (elements) of a staged tile: 16 bytes of padding per row
+template <typename T, int DH> struct Pitch { static constexpr int LDS = DH + 16 / (int)sizeof(T); };
 __device__ __forceinline__ void cpa16(void* dst, const void* src, bool valid) {
   const int sz = valid ? 16 : 0;
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(sz) : "memory");
@@ -37,98 +48,192 @@ __device__ __forceinline__ void cpa_commit() { asm volatile("cp.async.commit_gro
 template <int N>
 __device__ __forceinline__ void cpa_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// stage a [ROWS x DH] tile (row stride ld floats in global) into smem with row pitch DH+4;
+// stage a [ROWS x DH] tile (row stride ld elements in global) into smem with row pitch Pitch::LDS;
 // rows >= nvalid are zero-filled
-template <int DH, int ROWS, int THREADS>
-__device__ __forceinline__ void load_tile(float* s, const float* g, long long ld, int row0, int nvalid, int tid) {
-  constexpr int V = DH / 4;
-  constexpr int LDS = DH + 4;
+template <int DH, int ROWS, int THREADS, typename T>
+__device__ __forceinline__ void load_tile(T* s, const T* g, long long ld, int row0, int nvalid, int tid) {
+  constexpr int E = 16 / (int)sizeof(T);   // elements per 16-byte chunk
+  constexpr int V = DH / E;
+  constexpr int LDS = Pitch<T, DH>::LDS;
 #pragma unroll
   for (int i = tid; i < ROWS * V; i += THREADS) {
-    const int r = i / V, c = (i % V) * 4;
+    const int r = i / V, c = (i % V) * E;
     const bool ok = row0 + r < nvalid;
     cpa16(s + r * LDS + c, g + (long long)(ok ? row0 + r : 0) * ld + c, ok);
   }
 }
 
 // A-operand fragments of a 16 x DH row block read straight from global memory (row stride ld)
-template <int DH>
-__device__ __forceinline__ void load_a_frags(uint32_t (&f)[DH / 8][4], const float* base, long long ld, int row_lo,
+template <int DH, typename T>
+__device__ __forceinline__ void load_a_frags(uint32_t (&f)[DH / 8][4], const T* base, long long ld, int row_lo,
                                              int nvalid, int lane) {
   const int g = lane >> 2, t = lane & 3;
   const int r0 = row_lo + g, r1 = row_lo + g + 8;
-  const float* p0 = base + (long long)(r0 < nvalid ? r0 : 0) * ld;
-  const float* p1 = base + (long long)(r1 < nvalid ? r1 : 0) * ld;
+  const T* p0 = base + (long long)(r0 < nvalid ? r0 : 0) * ld;
+  const T* p1 = base + (long long)(r1 < nvalid ? r1 : 0) * ld;
   const bool ok0 = r0 < nvalid, ok1 = r1 < nvalid;
 #pragma unroll
   for (int k = 0; k < DH / 8; ++k) {
-    f[k][0] = ok0 ? __float_as_uint(p0[k * 8 + t]) : 0u;
-    f[k][1] = ok1 ? __float_as_uint(p1[k * 8 + t]) : 0u;
-    f[k][2] = ok0 ? __float_as_uint(p0[k * 8 + t + 4]) : 0u;
-    f[k][3] = ok1 ? __float_as_uint(p1[k * 8 + t + 4]) : 0u;
+    f[k][0] = ok0 ? ldbits(p0 + k * 8 + t) : 0u;
+    f[k][1] = ok1 ? ldbits(p1 + k * 8 + t) : 0u;
+    f[k][2] = ok0 ? ldbits(p0 + k * 8 + t + 4) : 0u;
+    f[k][3] = ok1 ? ldbits(p1 + k * 8 + t + 4) : 0u;
   }
 }
 
 // acc[nt] (16 x 8 each, nt over 64/8 column tiles) += A(16 x DH, regs) . T^T where T is a smem
 // tile [64][DH+4] whose rows are the output columns ("K-like" read: b = T[n0+g][k0+t])
-template <int DH>
-__device__ __forceinline__ void mma_rows_x_tileT(float (&acc)[8][4], const uint32_t (&a)[DH / 8][4], const float* T, int lane) {
-  constexpr int LDS = DH + 4;
+template <int DH, int PASSES, typename T>
+__device__ __forceinline__ void mma_rows_x_tileT(float (&acc)[8][4], const uint32_t (&a)[DH / 8][4], const T* Ts, int lane) {
+  constexpr int LDS = Pitch<T, DH>::LDS;
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int k = 0; k < DH / 8; ++k)
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
-      const float* p = T + (nt * 8 + g) * LDS + k * 8 + t;
-      mma_3xtf32(acc[nt], a[k], __float_as_uint(p[0]), __float_as_uint(p[4]));
+      const T* p = Ts + (nt * 8 + g) * LDS + k * 8 + t;
+      mma_x<PASSES>(acc[nt], a[k], ldbits(p), ldbits(p + 4));
     }
 }
 // acc[dt] (16 x 8 each, dt over DH/8 column tiles) += P(16 x 64, given as accumulator-layout
 // fragments, full fp32) . T where T is a smem tile [64][DH+4] whose rows are the
 // contraction index ("V-like" read).  Accumulator columns (2t, 2t+1) of each 8-wide tile serve
 // as k-slots (t, t+4), so the tile rows are read in the matching order 2t, 2t+1.
-template <int DH>
-__device__ __forceinline__ void mma_p_x_tile(float (&acc)[DH / 8][4], const uint32_t (&p)[8][4], const float* T, int lane) {
-  constexpr int LDS = DH + 4;
+template <int DH, int PASSES, typename T>
+__device__ __forceinline__ void mma_p_x_tile(float (&acc)[DH / 8][4], const uint32_t (&p)[8][4], const T* Ts, int lane) {
+  constexpr int LDS = Pitch<T, DH>::LDS;
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int kt = 0; kt < 8; ++kt)
 #pragma unroll
     for (int dt = 0; dt < DH / 8; ++dt) {
-      const float* q = T + (kt * 8 + 2 * t) * LDS + dt * 8 + g;
-      mma_3xtf32(acc[dt], p[kt], __float_as_uint(q[0]), __float_as_uint(q[LDS]));
+      const T* q = Ts + (kt * 8 + 2 * t) * LDS + dt * 8 + g;
+      mma_x<PASSES>(acc[dt], p[kt], ldbits(q), ldbits(q + LDS));
     }
 }
-// accumulator (c0,c1,c2,c3) -> A fragment (a0,a1,a2,a3) = (c0,c2,c1,c3), kept in full fp32 (split at the MMA)
+// accumulator (c0,c1,c2,c3) -> A fragment (a0,a1,a2,a3) = (c0,c2,c1,c3): kept in full fp32 for the 3-pass product
+// (split at the MMA), rounded to nearest tf32 for the single pass
+template <int PASSES>
 __device__ __forceinline__ void acc_to_a(uint32_t (&a)[4], float c0, float c1, float c2, float c3) {
+  if constexpr (PASSES == 1) { c0 = round_tf32(c0); c1 = round_tf32(c1); c2 = round_tf32(c2); c3 = round_tf32(c3); }
   a[0] = __float_as_uint(c0); a[1] = __float_as_uint(c2); a[2] = __float_as_uint(c1); a[3] = __float_as_uint(c3);
 }
+// two adjacent output elements: fp32 (optionally tf32-rounded) or fp16 (saturating)
+template <int OUT16>
+__device__ __forceinline__ void store2(void* base, long long off, float a, float b, int round_out) {
+  if constexpr (OUT16) {
+    *reinterpret_cast<uint32_t*>(static_cast<__half*>(base) + off) = pack_half2_sat(a, b);
+  } else {
+    if (round_out) { a = round_tf32(a); b = round_tf32(b); }
+    *reinterpret_cast<float2*>(static_cast<float*>(base) + off) = make_float2(a, b);
+  }
+}
+
+// The operand path of the kernels below.  fp32 storage: tf32 m16n8k8 (one or three passes), A fragments [DH/8][4],
+// P / dS fragments [8][4].  fp16 storage: f16 m16n8k16 with ldmatrix (B operands of both orientations straight from the
+// staged tiles), A fragments [DH/16][4], P / dS fragments packed to fp16 pairs [4][4].
+template <int DH, int PASSES, int IN16> struct Ops;
+template <int DH, int PASSES> struct Ops<DH, PASSES, 0> {
+  using T = float;
+  using QF = uint32_t[DH / 8][4];
+  using PF = uint32_t[8][4];
+  static __device__ __forceinline__ void load_a(QF& f, const T* base, long long ld, int row_lo, int nvalid, int lane) {
+    load_a_frags<DH>(f, base, ld, row_lo, nvalid, lane);
+  }
+  static __device__ __forceinline__ void rows_x_tileT(float (&acc)[8][4], const QF& a, const T* Ts, int lane) {
+    mma_rows_x_tileT<DH, PASSES>(acc, a, Ts, lane);
+  }
+  static __device__ __forceinline__ void p_x_tile(float (&acc)[DH / 8][4], const PF& pf, const T* Ts, int lane) {
+    mma_p_x_tile<DH, PASSES>(acc, pf, Ts, lane);
+  }
+  static __device__ __forceinline__ void set_p(PF& pf, int nt, float c0, float c1, float c2, float c3) {
+    acc_to_a<PASSES>(pf[nt], c0, c1, c2, c3);
+  }
+};
+template <int DH> struct Ops<DH, 1, 1> {
+  using T = __half;
+  using QF = uint32_t[DH / 16][4];
+  using PF = uint32_t[4][4];
+  static constexpr int LDS = Pitch<T, DH>::LDS;
+  // A fragments of a 16 x DH row block from global memory: a0 (row g, k 2t..2t+1), a1 (row g+8), a2 / a3 (k + 8)
+  static __device__ __forceinline__ void load_a(QF& f, const T* base, long long ld, int row_lo, int nvalid, int lane) {
+    const int g = lane >> 2, t = lane & 3;
+    const int r0 = row_lo + g, r1 = row_lo + g + 8;
+    const bool ok0 = r0 < nvalid, ok1 = r1 < nvalid;
+    const T* p0 = base + (long long)(ok0 ? r0 : 0) * ld + 2 * t;
+    const T* p1 = base + (long long)(ok1 ? r1 : 0) * ld + 2 * t;
+#pragma unroll
+    for (int kc = 0; kc < DH / 16; ++kc) {
+      f[kc][0] = ok0 ? *reinterpret_cast<const uint32_t*>(p0 + kc * 16) : 0u;
+      f[kc][1] = ok1 ? *reinterpret_cast<const uint32_t*>(p1 + kc * 16) : 0u;
+      f[kc][2] = ok0 ? *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8) : 0u;
+      f[kc][3] = ok1 ? *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8) : 0u;
+    }
+  }
+  // acc[nt] += A . T^T, T a staged [64][DH] tile whose rows are the output columns: ldmatrix (no transpose) gives
+  // b0 / b1 of two n8 tiles per x4 load
+  static __device__ __forceinline__ void rows_x_tileT(float (&acc)[8][4], const QF& a, const T* Ts, int lane) {
+    const int lr = lane & 7, lj = lane >> 3;
+    const uint32_t base = smem_u32(Ts);
+#pragma unroll
+    for (int kc = 0; kc < DH / 16; ++kc)
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t v[4];
+        ldsm_x4(base + (uint32_t)(((np * 16 + (lj >> 1) * 8 + lr) * LDS + kc * 16 + (lj & 1) * 8) * 2), v);
+        mma_f16(acc[2 * np], a[kc], v[0], v[1]);
+        mma_f16(acc[2 * np + 1], a[kc], v[2], v[3]);
+      }
+  }
+  // acc[dt] += P . T, T a staged [64][DH] tile whose rows are the contraction index: ldmatrix.trans
+  static __device__ __forceinline__ void p_x_tile(float (&acc)[DH / 8][4], const PF& pf, const T* Ts, int lane) {
+    const int lr = lane & 7, lj = lane >> 3;
+    const uint32_t base = smem_u32(Ts);
+#pragma unroll
+    for (int kc = 0; kc < 4; ++kc)
+#pragma unroll
+      for (int dp = 0; dp < DH / 16; ++dp) {
+        uint32_t v[4];
+        ldsm_x4_t(base + (uint32_t)(((kc * 16 + (lj & 1) * 8 + lr) * LDS + dp * 16 + (lj >> 1) * 8) * 2), v);
+        mma_f16(acc[2 * dp], pf[kc], v[0], v[1]);
+        mma_f16(acc[2 * dp + 1], pf[kc], v[2], v[3]);
+      }
+  }
+  // accumulator tile nt (c0, c1: row g; c2, c3: row g + 8) -> half of the k16 A fragment kc = nt / 2
+  static __device__ __forceinline__ void set_p(PF& pf, int nt, float c0, float c1, float c2, float c3) {
+    pf[nt >> 1][(nt & 1) * 2] = pack_half2_sat(c0, c1);
+    pf[nt >> 1][(nt & 1) * 2 + 1] = pack_half2_sat(c2, c3);
+  }
+};
 
 // ---------------------------------------------------------------------------------------------
 // forward: grid (ceil(N/128), heads, B), 256 threads = 8 warps x 16 query rows
 // ---------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, int PASSES, int IN16, int OUT16>
 __global__ void __launch_bounds__(256)
-attn_exact_fwd_kernel(const float* __restrict__ qkv, float* __restrict__ out, float* __restrict__ lse, int N, int heads,
-                float scale, int cond) {
-  constexpr int LDS = DH + 4;
+attn_fwd_kernel(const void* __restrict__ qkv_, void* __restrict__ out, float* __restrict__ lse, int N, int heads,
+                float scale, int cond, int round_out) {
+  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  const T* qkv = static_cast<const T*>(qkv_);
+  constexpr int LDS = Pitch<T, DH>::LDS;
   constexpr int TILE = 64 * LDS;
-  extern __shared__ __align__(16) float sm[];   // K[2][TILE], V[2][TILE]
-  float* Ks = sm;
-  float* Vs = sm + 2 * TILE;
+  extern __shared__ __align__(16) uint8_t sm_raw[];   // K[2][TILE], V[2][TILE]
+  T* Ks = reinterpret_cast<T*>(sm_raw);
+  T* Vs = Ks + 2 * TILE;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   const int h = blockIdx.y, b = blockIdx.z;
   const int inner = heads * DH;
   const long long ld = 3ll * inner;
-  const float* qbase = qkv + (long long)b * N * ld + h * DH;
-  const float* kbase = qbase + inner;
-  const float* vbase = qbase + 2 * inner;
+  const T* qbase = qkv + (long long)b * N * ld + h * DH;
+  const T* kbase = qbase + inner;
+  const T* vbase = qbase + 2 * inner;
   const int q0 = blockIdx.x * 128 + warp * 16;
   const float c = scale * kLog2e;
 
-  uint32_t qf[DH / 8][4];
-  load_a_frags<DH>(qf, qbase, ld, q0, N, lane);
+  using Op = Ops<DH, PASSES, IN16>;
+  typename Op::QF qf;
+  Op::load_a(qf, qbase, ld, q0, N, lane);
 
   float o[DH / 8][4];
 #pragma unroll
@@ -157,7 +262,7 @@ attn_exact_fwd_kernel(const float* __restrict__ qkv, float* __restrict__ out, fl
     float s[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
-    mma_rows_x_tileT<DH>(s, qf, Ks + buf * TILE, lane);
+    Op::rows_x_tileT(s, qf, Ks + buf * TILE, lane);
     if ((j + 1) * 64 > N) {
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
@@ -190,28 +295,26 @@ attn_exact_fwd_kernel(const float* __restrict__ qkv, float* __restrict__ out, fl
     l0 *= al0; l1 *= al1;
 #pragma unroll
     for (int i = 0; i < DH / 8; ++i) { o[i][0] *= al0; o[i][1] *= al0; o[i][2] *= al1; o[i][3] *= al1; }
-    uint32_t pf[8][4];
+    typename Op::PF pf;
     const float mc0 = m0 * c, mc1 = m1 * c;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const float p0 = exp2f(s[nt][0] * c - mc0), p1 = exp2f(s[nt][1] * c - mc0);
       const float p2 = exp2f(s[nt][2] * c - mc1), p3 = exp2f(s[nt][3] * c - mc1);
       l0 += p0 + p1; l1 += p2 + p3;
-      acc_to_a(pf[nt], p0, p1, p2, p3);
+      Op::set_p(pf, nt, p0, p1, p2, p3);
     }
-    mma_p_x_tile<DH>(o, pf, Vs + buf * TILE, lane);
+    Op::p_x_tile(o, pf, Vs + buf * TILE, lane);
   }
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
   const float inv0 = 1.f / l0, inv1 = 1.f / l1;
   const int r0 = q0 + g, r1 = q0 + g + 8;
-  float* ob = out + (long long)b * N * inner + h * DH;
+  const long long ob = (long long)b * N * inner + h * DH;
 #pragma unroll
   for (int dt = 0; dt < DH / 8; ++dt) {
-    float2 a = make_float2(o[dt][0] * inv0, o[dt][1] * inv0);
-    float2 bb = make_float2(o[dt][2] * inv1, o[dt][3] * inv1);
-    if (r0 < N) *reinterpret_cast<float2*>(ob + (long long)r0 * inner + dt * 8 + 2 * t) = a;
-    if (r1 < N) *reinterpret_cast<float2*>(ob + (long long)r1 * inner + dt * 8 + 2 * t) = bb;
+    if (r0 < N) store2<OUT16>(out, ob + (long long)r0 * inner + dt * 8 + 2 * t, o[dt][0] * inv0, o[dt][1] * inv0, round_out);
+    if (r1 < N) store2<OUT16>(out, ob + (long long)r1 * inner + dt * 8 + 2 * t, o[dt][2] * inv1, o[dt][3] * inv1, round_out);
   }
   if (t == 0) {
     float* lb = lse + ((long long)b * heads + h) * N;
@@ -225,32 +328,37 @@ attn_exact_fwd_kernel(const float* __restrict__ qkv, float* __restrict__ out, fl
 // Works on transposed score tiles S^T[key, query] so that P^T / dS^T come out of the tensor
 // cores already in A-operand position for dV += P^T dO and dK += dS^T Q.
 // ---------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, int PASSES, int IN16, int OUT16>
 __global__ void __launch_bounds__(128)
-attn_exact_bwd_dkv_kernel(const float* __restrict__ qkv, const float* __restrict__ dout, const float* __restrict__ lse,
-                    const float* __restrict__ delta, float* __restrict__ dqkv, int N, int heads, float scale, int cond) {
-  constexpr int LDS = DH + 4;
+attn_bwd_dkv_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_, const float* __restrict__ lse,
+                    const float* __restrict__ delta, void* __restrict__ dqkv, const float* __restrict__ out_scale, int N,
+                    int heads, float scale, int cond, int round_out) {
+  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  const T* qkv = static_cast<const T*>(qkv_);
+  const T* dout = static_cast<const T*>(dout_);
+  constexpr int LDS = Pitch<T, DH>::LDS;
   constexpr int TILE = 64 * LDS;
-  extern __shared__ __align__(16) float sm[];   // Q[2][TILE], dO[2][TILE], lse[2][64], delta[2][64]
-  float* Qs = sm;
-  float* Ds = sm + 2 * TILE;
-  float* Ls = sm + 4 * TILE;
+  extern __shared__ __align__(16) uint8_t sm_raw[];   // Q[2][TILE], dO[2][TILE], lse[2][64], delta[2][64]
+  T* Qs = reinterpret_cast<T*>(sm_raw);
+  T* Ds = Qs + 2 * TILE;
+  float* Ls = reinterpret_cast<float*>(Ds + 2 * TILE);
   float* Es = Ls + 128;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   const int h = blockIdx.y, b = blockIdx.z;
   const int inner = heads * DH;
   const long long ld = 3ll * inner;
-  const float* qbase = qkv + (long long)b * N * ld + h * DH;
-  const float* dobase = dout + (long long)b * N * inner + h * DH;
+  const T* qbase = qkv + (long long)b * N * ld + h * DH;
+  const T* dobase = dout + (long long)b * N * inner + h * DH;
   const float* lb = lse + ((long long)b * heads + h) * N;
   const float* eb = delta + ((long long)b * heads + h) * N;
   const int k0 = blockIdx.x * 64 + warp * 16;
   const float c = scale * kLog2e;
 
-  uint32_t kf[DH / 8][4], vf[DH / 8][4];
-  load_a_frags<DH>(kf, qbase + inner, ld, k0, N, lane);
-  load_a_frags<DH>(vf, qbase + 2 * inner, ld, k0, N, lane);
+  using Op = Ops<DH, PASSES, IN16>;
+  typename Op::QF kf, vf;
+  Op::load_a(kf, qbase + inner, ld, k0, N, lane);
+  Op::load_a(vf, qbase + 2 * inner, ld, k0, N, lane);
   float dk[DH / 8][4], dv[DH / 8][4];
 #pragma unroll
   for (int i = 0; i < DH / 8; ++i) { dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.f; dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f; }
@@ -277,13 +385,13 @@ attn_exact_bwd_dkv_kernel(const float* __restrict__ qkv, const float* __restrict
     cpa_wait<0>();
     __syncthreads();
     if (j + 1 < ntiles) stage(j + 1, buf ^ 1);
-    const float* Q = Qs + buf * TILE;
-    const float* dO = Ds + buf * TILE;
+    const T* Q = Qs + buf * TILE;
+    const T* dO = Ds + buf * TILE;
     float s[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
-    mma_rows_x_tileT<DH>(s, kf, Q, lane);            // S^T = K Q^T
-    uint32_t pf[8][4];
+    Op::rows_x_tileT(s, kf, Q, lane);                // S^T = K Q^T
+    typename Op::PF pf;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const float la = Ls[buf * 64 + nt * 8 + 2 * t], lbb = Ls[buf * 64 + nt * 8 + 2 * t + 1];
@@ -296,35 +404,35 @@ attn_exact_bwd_dkv_kernel(const float* __restrict__ qkv, const float* __restrict
         if (kr1 > va) s[nt][2] = 0.f;
         if (kr1 > vb) s[nt][3] = 0.f;
       }
-      acc_to_a(pf[nt], s[nt][0], s[nt][1], s[nt][2], s[nt][3]);
+      Op::set_p(pf, nt, s[nt][0], s[nt][1], s[nt][2], s[nt][3]);
     }
-    mma_p_x_tile<DH>(dv, pf, dO, lane);              // dV += P^T dO
+    Op::p_x_tile(dv, pf, dO, lane);                  // dV += P^T dO
     float dp[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f; }
-    mma_rows_x_tileT<DH>(dp, vf, dO, lane);          // dP^T = V dO^T
+    Op::rows_x_tileT(dp, vf, dO, lane);              // dP^T = V dO^T
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const float ea = Es[buf * 64 + nt * 8 + 2 * t], ebb = Es[buf * 64 + nt * 8 + 2 * t + 1];
-      acc_to_a(pf[nt], s[nt][0] * (dp[nt][0] - ea), s[nt][1] * (dp[nt][1] - ebb), s[nt][2] * (dp[nt][2] - ea),
-               s[nt][3] * (dp[nt][3] - ebb));
+      Op::set_p(pf, nt, s[nt][0] * (dp[nt][0] - ea), s[nt][1] * (dp[nt][1] - ebb), s[nt][2] * (dp[nt][2] - ea),
+                s[nt][3] * (dp[nt][3] - ebb));
     }
-    mma_p_x_tile<DH>(dk, pf, Q, lane);               // dK += dS^T Q
+    Op::p_x_tile(dk, pf, Q, lane);                   // dK += dS^T Q
   }
   const int r0 = k0 + g, r1 = k0 + g + 8;
-  float* dkb = dqkv + (long long)b * N * ld + inner + h * DH;
-  float* dvb = dkb + inner;
+  const long long dkb = (long long)b * N * ld + inner + h * DH;
+  const long long dvb = dkb + inner;
+  const float vm = out_scale ? __ldg(out_scale) : 1.f;     // fp16 output: the gradient scale it travels with
+  const float km = scale * vm;
 #pragma unroll
   for (int dt = 0; dt < DH / 8; ++dt) {
-    float2 a = make_float2(dk[dt][0] * scale, dk[dt][1] * scale), a2 = make_float2(dk[dt][2] * scale, dk[dt][3] * scale);
-    float2 v = make_float2(dv[dt][0], dv[dt][1]), v2 = make_float2(dv[dt][2], dv[dt][3]);
     if (r0 < N) {
-      *reinterpret_cast<float2*>(dkb + (long long)r0 * ld + dt * 8 + 2 * t) = a;
-      *reinterpret_cast<float2*>(dvb + (long long)r0 * ld + dt * 8 + 2 * t) = v;
+      store2<OUT16>(dqkv, dkb + (long long)r0 * ld + dt * 8 + 2 * t, dk[dt][0] * km, dk[dt][1] * km, round_out);
+      store2<OUT16>(dqkv, dvb + (long long)r0 * ld + dt * 8 + 2 * t, dv[dt][0] * vm, dv[dt][1] * vm, round_out);
     }
     if (r1 < N) {
-      *reinterpret_cast<float2*>(dkb + (long long)r1 * ld + dt * 8 + 2 * t) = a2;
-      *reinterpret_cast<float2*>(dvb + (long long)r1 * ld + dt * 8 + 2 * t) = v2;
+      store2<OUT16>(dqkv, dkb + (long long)r1 * ld + dt * 8 + 2 * t, dk[dt][2] * km, dk[dt][3] * km, round_out);
+      store2<OUT16>(dqkv, dvb + (long long)r1 * ld + dt * 8 + 2 * t, dv[dt][2] * vm, dv[dt][3] * vm, round_out);
     }
   }
 }
@@ -332,24 +440,28 @@ attn_exact_bwd_dkv_kernel(const float* __restrict__ qkv, const float* __restrict
 // ---------------------------------------------------------------------------------------------
 // backward, query side: grid (ceil(N/64), heads, B), 128 threads = 4 warps x 16 queries
 // ---------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, int PASSES, int IN16, int OUT16>
 __global__ void __launch_bounds__(128)
-attn_exact_bwd_dq_kernel(const float* __restrict__ qkv, const float* __restrict__ dout, const float* __restrict__ lse,
-                   const float* __restrict__ delta, float* __restrict__ dqkv, int N, int heads, float scale, int cond) {
-  constexpr int LDS = DH + 4;
+attn_bwd_dq_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_, const float* __restrict__ lse,
+                   const float* __restrict__ delta, void* __restrict__ dqkv, const float* __restrict__ out_scale, int N,
+                   int heads, float scale, int cond, int round_out) {
+  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  const T* qkv = static_cast<const T*>(qkv_);
+  const T* dout = static_cast<const T*>(dout_);
+  constexpr int LDS = Pitch<T, DH>::LDS;
   constexpr int TILE = 64 * LDS;
-  extern __shared__ __align__(16) float sm[];   // K[2][TILE], V[2][TILE]
-  float* Ks = sm;
-  float* Vs = sm + 2 * TILE;
+  extern __shared__ __align__(16) uint8_t sm_raw[];   // K[2][TILE], V[2][TILE]
+  T* Ks = reinterpret_cast<T*>(sm_raw);
+  T* Vs = Ks + 2 * TILE;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   const int h = blockIdx.y, b = blockIdx.z;
   const int inner = heads * DH;
   const long long ld = 3ll * inner;
-  const float* qbase = qkv + (long long)b * N * ld + h * DH;
-  const float* kbase = qbase + inner;
-  const float* vbase = qbase + 2 * inner;
-  const float* dobase = dout + (long long)b * N * inner + h * DH;
+  const T* qbase = qkv + (long long)b * N * ld + h * DH;
+  const T* kbase = qbase + inner;
+  const T* vbase = qbase + 2 * inner;
+  const T* dobase = dout + (long long)b * N * inner + h * DH;
   const int q0 = blockIdx.x * 64 + warp * 16;
   const float c = scale * kLog2e;
   const int r0 = q0 + g, r1 = q0 + g + 8;
@@ -358,9 +470,10 @@ attn_exact_bwd_dq_kernel(const float* __restrict__ qkv, const float* __restrict_
   const float lse0 = r0 < N ? lb[r0] * kLog2e : INFINITY, lse1 = r1 < N ? lb[r1] * kLog2e : INFINITY;
   const float e0 = r0 < N ? eb[r0] : 0.f, e1 = r1 < N ? eb[r1] : 0.f;
 
-  uint32_t qf[DH / 8][4], dof[DH / 8][4];
-  load_a_frags<DH>(qf, qbase, ld, q0, N, lane);
-  load_a_frags<DH>(dof, dobase, inner, q0, N, lane);
+  using Op = Ops<DH, PASSES, IN16>;
+  typename Op::QF qf, dof;
+  Op::load_a(qf, qbase, ld, q0, N, lane);
+  Op::load_a(dof, dobase, inner, q0, N, lane);
   float dq[DH / 8][4];
 #pragma unroll
   for (int i = 0; i < DH / 8; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
@@ -384,54 +497,57 @@ attn_exact_bwd_dq_kernel(const float* __restrict__ qkv, const float* __restrict_
     float s[8][4], dp[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f; }
-    mma_rows_x_tileT<DH>(s, qf, Ks + buf * TILE, lane);     // S = Q K^T
-    mma_rows_x_tileT<DH>(dp, dof, Vs + buf * TILE, lane);   // dP = dO V^T
-    uint32_t pf[8][4];
+    Op::rows_x_tileT(s, qf, Ks + buf * TILE, lane);     // S = Q K^T
+    Op::rows_x_tileT(dp, dof, Vs + buf * TILE, lane);   // dP = dO V^T
+    typename Op::PF pf;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const int key = j * 64 + nt * 8 + 2 * t;
       const bool ka = key < N, kb = key + 1 < N;
       const float p0 = (ka && key <= lim0) ? exp2f(s[nt][0] * c - lse0) : 0.f, p1 = (kb && key + 1 <= lim0) ? exp2f(s[nt][1] * c - lse0) : 0.f;
       const float p2 = (ka && key <= lim1) ? exp2f(s[nt][2] * c - lse1) : 0.f, p3 = (kb && key + 1 <= lim1) ? exp2f(s[nt][3] * c - lse1) : 0.f;
-      acc_to_a(pf[nt], p0 * (dp[nt][0] - e0), p1 * (dp[nt][1] - e0), p2 * (dp[nt][2] - e1), p3 * (dp[nt][3] - e1));
+      Op::set_p(pf, nt, p0 * (dp[nt][0] - e0), p1 * (dp[nt][1] - e0), p2 * (dp[nt][2] - e1), p3 * (dp[nt][3] - e1));
     }
-    mma_p_x_tile<DH>(dq, pf, Ks + buf * TILE, lane);        // dQ += dS K
+    Op::p_x_tile(dq, pf, Ks + buf * TILE, lane);        // dQ += dS K
   }
-  float* dqb = dqkv + (long long)b * N * ld + h * DH;
+  const long long dqb = (long long)b * N * ld + h * DH;
+  const float qm = scale * (out_scale ? __ldg(out_scale) : 1.f);
 #pragma unroll
   for (int dt = 0; dt < DH / 8; ++dt) {
-    float2 a = make_float2(dq[dt][0] * scale, dq[dt][1] * scale), a2 = make_float2(dq[dt][2] * scale, dq[dt][3] * scale);
-    if (r0 < N) *reinterpret_cast<float2*>(dqb + (long long)r0 * ld + dt * 8 + 2 * t) = a;
-    if (r1 < N) *reinterpret_cast<float2*>(dqb + (long long)r1 * ld + dt * 8 + 2 * t) = a2;
+    if (r0 < N) store2<OUT16>(dqkv, dqb + (long long)r0 * ld + dt * 8 + 2 * t, dq[dt][0] * qm, dq[dt][1] * qm, round_out);
+    if (r1 < N) store2<OUT16>(dqkv, dqb + (long long)r1 * ld + dt * 8 + 2 * t, dq[dt][2] * qm, dq[dt][3] * qm, round_out);
   }
 }
 
 
 // ---------------------------------------------------------------------------------------------
-template <int DH>
-static int exact_fwd_launch(const float* qkv, float* out, float* lse, int B, int N, int heads, float scale, int cond, cudaStream_t s) {
-  constexpr size_t smem = 4 * 64 * (DH + 4) * sizeof(float);
-  auto kern = attn_exact_fwd_kernel<DH>;
+template <int DH, int PASSES, int IN16, int OUT16>
+static int fwd_launch(const void* qkv, void* out, float* lse, int B, int N, int heads, float scale, int cond, int round_out,
+                      cudaStream_t s) {
+  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  constexpr size_t smem = 4 * 64 * Pitch<T, DH>::LDS * sizeof(T);
+  auto kern = attn_fwd_kernel<DH, PASSES, IN16, OUT16>;
   B200_CONFIGURE_SMEM_ONCE(kern, smem);
-  kern<<<dim3((N + 127) / 128, heads, B), 256, smem, s>>>(qkv, out, lse, N, heads, scale, cond);
-  B200_LAUNCH_OK("attn_exact_fwd_kernel");
+  kern<<<dim3((N + 127) / 128, heads, B), 256, smem, s>>>(qkv, out, lse, N, heads, scale, cond, round_out);
+  B200_LAUNCH_OK("attn_fwd_kernel");
   return 0;
 }
 
-template <int DH>
-static int exact_bwd_launch(const float* qkv, const float* dout, const float* lse, const float* delta, float* dqkv, int B,
-                            int N, int heads, float scale, int cond, cudaStream_t s) {
-  constexpr size_t smem_kv = (4 * 64 * (DH + 4) + 256) * sizeof(float);
-  constexpr size_t smem_q = 4 * 64 * (DH + 4) * sizeof(float);
-  auto k1 = attn_exact_bwd_dkv_kernel<DH>;
-  auto k2 = attn_exact_bwd_dq_kernel<DH>;
+template <int DH, int PASSES, int IN16, int OUT16>
+static int bwd_launch(const void* qkv, const void* dout, const float* lse, const float* delta, void* dqkv, const float* out_scale,
+                      int B, int N, int heads, float scale, int cond, int round_out, cudaStream_t s) {
+  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  constexpr size_t smem_kv = 4 * 64 * Pitch<T, DH>::LDS * sizeof(T) + 256 * sizeof(float);
+  constexpr size_t smem_q = 4 * 64 * Pitch<T, DH>::LDS * sizeof(T);
+  auto k1 = attn_bwd_dkv_kernel<DH, PASSES, IN16, OUT16>;
+  auto k2 = attn_bwd_dq_kernel<DH, PASSES, IN16, OUT16>;
   B200_CONFIGURE_SMEM_ONCE(k1, smem_kv);
   B200_CONFIGURE_SMEM_ONCE(k2, smem_q);
   const dim3 grid((N + 63) / 64, heads, B);
-  k1<<<grid, 128, smem_kv, s>>>(qkv, dout, lse, delta, dqkv, N, heads, scale, cond);
-  B200_LAUNCH_OK("attn_exact_bwd_dkv_kernel");
-  k2<<<grid, 128, smem_q, s>>>(qkv, dout, lse, delta, dqkv, N, heads, scale, cond);
-  B200_LAUNCH_OK("attn_exact_bwd_dq_kernel");
+  k1<<<grid, 128, smem_kv, s>>>(qkv, dout, lse, delta, dqkv, out_scale, N, heads, scale, cond, round_out);
+  B200_LAUNCH_OK("attn_bwd_dkv_kernel");
+  k2<<<grid, 128, smem_q, s>>>(qkv, dout, lse, delta, dqkv, out_scale, N, heads, scale, cond, round_out);
+  B200_LAUNCH_OK("attn_bwd_dq_kernel");
   return 0;
 }
 
@@ -439,27 +555,74 @@ static int exact_bwd_launch(const float* qkv, const float* dout, const float* ls
 int attention_delta(const void* out, int out_half, const void* dout, int dout_half, float* delta, int B, int N, int heads, int dh,
                     cudaStream_t stream);
 
-// cond_len < 0: no mask (stage 1).  cond_len >= 0: the stage-2 mask, causal with a fully visible prefix of cond_len tokens.
-int attention_exact_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
-                            int cond_len, cudaStream_t stream) {
+static int check_problem(const void* qkv, int B, int N, int heads, int dh, int cond_len) {
   B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
   B200_CHECK_ARG(dh == 64 || dh == 32, "attention: dim_head must be 32 or 64 (got %d)", dh);
   B200_CHECK_ARG(B <= 65535 && heads <= 65535, "attention: grid too large");
   B200_CHECK_ARG(cond_len <= N, "attention: cond_len %d exceeds the sequence length %d", cond_len, N);
-  if (dh == 64) return exact_fwd_launch<64>(qkv, out, lse, B, N, heads, scale, cond_len, stream);
-  return exact_fwd_launch<32>(qkv, out, lse, B, N, heads, scale, cond_len, stream);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0, "attention: qkv must be 16-byte aligned");
+  return 0;
+}
+
+// cond_len < 0: no mask (stage 1).  cond_len >= 0: the stage-2 mask, causal with a fully visible prefix of cond_len tokens.
+int attention_exact_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
+                            int cond_len, cudaStream_t stream) {
+  if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
+  if (dh == 64) return fwd_launch<64, 3, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
+  return fwd_launch<32, 3, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
 }
 
 int attention_exact_backward(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv, float* delta,
                              int B, int N, int heads, int dh, float scale, int cond_len, cudaStream_t stream) {
-  B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
-  B200_CHECK_ARG(cond_len <= N, "attention: cond_len %d exceeds the sequence length %d", cond_len, N);
-  B200_CHECK_ARG(dh == 64 || dh == 32, "attention: dim_head must be 32 or 64 (got %d)", dh);
-  B200_CHECK_ARG(B <= 65535 && heads <= 65535, "attention: grid too large");
+  if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
   int rc = attention_delta(out, 0, dout, 0, delta, B, N, heads, dh, stream);
   if (rc) return rc;
-  if (dh == 64) return exact_bwd_launch<64>(qkv, dout, lse, delta, dqkv, B, N, heads, scale, cond_len, stream);
-  return exact_bwd_launch<32>(qkv, dout, lse, delta, dqkv, B, N, heads, scale, cond_len, stream);
+  if (dh == 64) return bwd_launch<64, 3, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
+  return bwd_launch<32, 3, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
+}
+
+// tf32 core: fp32 q/k/v (tf32-rounded by the GEMM that wrote them); O in fp32 (optionally tf32-rounded) or fp16
+int attention_forward_tc(const float* qkv, void* out, int out_half, float* lse, int B, int N, int heads, int dh, float scale,
+                         int round_out, int cond_len, cudaStream_t stream) {
+  if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
+  if (dh == 64) return out_half ? fwd_launch<64, 1, 0, 1>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
+                                : fwd_launch<64, 1, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
+  return out_half ? fwd_launch<32, 1, 0, 1>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
+                  : fwd_launch<32, 1, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
+}
+
+// delta must already hold rowsum(dO * O).  dqkv fp32 (optionally tf32-rounded) or, with out_half, fp16(dqkv * out_scale[0]).
+int attention_backward_tc(const float* qkv, const float* dout, const float* lse, const float* delta, void* dqkv, int out_half,
+                          const float* out_scale, int B, int N, int heads, int dh, float scale, int round_out, int cond_len,
+                          cudaStream_t stream) {
+  if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dout) & 15) == 0, "attention: dout must be 16-byte aligned");
+  if (dh == 64) return out_half ? bwd_launch<64, 1, 0, 1>(qkv, dout, lse, delta, dqkv, out_scale, B, N, heads, scale, cond_len, 0, stream)
+                                : bwd_launch<64, 1, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, round_out, stream);
+  return out_half ? bwd_launch<32, 1, 0, 1>(qkv, dout, lse, delta, dqkv, out_scale, B, N, heads, scale, cond_len, 0, stream)
+                  : bwd_launch<32, 1, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, round_out, stream);
+}
+
+// fp16 core (dim_head 64): q/k/v fp16 as the to_qkv GEMM stores them, O fp16.  Backward: dO fp16 carrying the power-of-two
+// gradient scale S of the backward segment (functional.py); delta, dS and the stored fp16 dq / dk / dv carry S too --
+// everything is linear in dO, nothing is rescaled here.
+int attention_f16_forward(const void* qkv, void* out, float* lse, int B, int N, int heads, int dh, float scale, cudaStream_t stream) {
+  B200_CHECK_ARG(dh == 64, "attention_f16: dim_head must be 64 (got %d); other head sizes use the tf32 core", dh);
+  if (int rc = check_problem(qkv, B, N, heads, dh, -1)) return rc;
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 15) == 0, "attention: out must be 16-byte aligned");
+  return fwd_launch<64, 1, 1, 1>(qkv, out, lse, B, N, heads, scale, -1, 0, stream);
+}
+
+int attention_f16_backward(const void* qkv, const void* out, const float* lse, const void* dout, void* dqkv, float* delta, int B, int N,
+                           int heads, int dh, float scale, cudaStream_t stream) {
+  B200_CHECK_ARG(dh == 64, "attention_f16: dim_head must be 64 (got %d)", dh);
+  if (int rc = check_problem(qkv, B, N, heads, dh, -1)) return rc;
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dout) & 15) == 0 && (reinterpret_cast<uintptr_t>(dqkv) & 15) == 0 &&
+                     (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+                 "attention: qkv/out/dout/dqkv must be 16-byte aligned");
+  int rc = attention_delta(out, 1, dout, 1, delta, B, N, heads, dh, stream);
+  if (rc) return rc;
+  return bwd_launch<64, 1, 1, 1>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, -1, 0, stream);
 }
 
 }  // namespace b200

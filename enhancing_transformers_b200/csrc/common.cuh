@@ -1,14 +1,13 @@
-// Shared device helpers: inline-PTX wrappers for mbarrier / TMA / tcgen05 (sm_100a only).
-// Hand-written; the encodings follow the PTX ISA as summarised in the Blackwell guides
-// (SM100 shared-memory matrix descriptor, instruction descriptor, 2-SM TMA peer-bit mask).
+// Shared device helpers: inline-PTX wrappers for mbarrier / TMA / mma.sync / ldmatrix (sm_90a).
+// Hand-written after the PTX ISA.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM100_ALL)
-#error "b200vq kernels must be compiled with -gencode arch=compute_100a,code=sm_100a"
+#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM90_ALL)
+#error "b200vq kernels must be compiled with -gencode arch=compute_90a,code=sm_90a"
 #endif
 
 namespace b200 {
@@ -55,13 +54,9 @@ struct PerDevice { bool done[kMaxDevices] = {}; int value[kMaxDevices] = {}; };
     }                                                                                                        \
   } while (0)
 // generic tiled tensor map (rank <= 5), cached.  elem_bytes: 4 = fp32, 2 = fp16;
-// swizzle: 0 = SWIZZLE_128B, 1 = SWIZZLE_128B_ATOM_32B (MN-major tf32 operands), 2 = SWIZZLE_64B, 3 = none
+// swizzle: 0 = SWIZZLE_128B, 1 = SWIZZLE_64B, 2 = none
 int make_tensor_map(CUtensorMap* out, const void* ptr, int elem_bytes, int rank, const unsigned long long* dims,
                     const unsigned long long* strides_bytes, const unsigned* box, int swizzle);
-inline int make_tensor_map_f32(CUtensorMap* out, const float* ptr, int rank, const unsigned long long* dims,
-                               const unsigned long long* strides_bytes, const unsigned* box, int swizzle_base32) {
-  return make_tensor_map(out, ptr, 4, rank, dims, strides_bytes, box, swizzle_base32);
-}
 
 #ifdef __CUDACC__
 // ------------------------------------------------------------------------------------------
@@ -73,37 +68,14 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 // 1024-byte alignment of the dynamic shared-memory base (SWIZZLE_128B atoms) as pointer arithmetic on the __shared__
 // symbol: a round trip through uintptr_t loses the address space and every later access becomes a generic LD / ST.
 __device__ __forceinline__ uint8_t* smem_align1024(uint8_t* raw) { return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u); }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-// One lane of a fully converged warp (the lowest).  Role warps keep their control flow warp-uniform
-// and gate only the issuing instructions with this: the compiler then keeps descriptors and loop
-// state in uniform registers instead of wrapping every tcgen05 / TMA instruction of a divergent
-// single-lane region in ELECT + R2UR sequences (measured: ~100 issue cycles per MMA otherwise).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 // round-to-nearest (ties away from zero, like cvt.rna.tf32.f32) fp32 -> tf32 (10-bit mantissa),
-// result kept in an fp32 container with the low 13 bits cleared.  Done with two integer ops on
-// the ALU pipe: cvt.rna.tf32 issues on the XU pipe (16 lanes/clk/SM, shared with ex2) and was the
-// measured bottleneck of the attention softmax warps.
+// result kept in an fp32 container with the low 13 bits cleared.  Two integer ops on the ALU pipe
+// instead of cvt.rna.tf32, which issues on the XU pipe shared with ex2.
 __device__ __forceinline__ float round_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-// Same rounding for a value that is consumed *only* as a tcgen05 kind::tf32 operand: the tensor core drops the
-// low 13 bits itself, so adding half an ulp is enough (one integer op).
-__device__ __forceinline__ uint32_t tf32_bits_for_mma(float x) { return __float_as_uint(x) + 0x1000u; }
 // tanh(x) = 1 - 2 / (exp(2x) + 1) with one ex2.approx and one rcp.approx (absolute error ~1e-7, far below the
-// tf32 rounding applied to the result).  libdevice's tanhf costs ~40 instructions and made the MLP-1 GEMM
-// epilogue-bound (1500 us vs 890 us for the same GEMM without the activation).
+// tf32 rounding applied to the result).  libdevice's tanhf costs ~40 instructions per element of the MLP-1 epilogue.
 __device__ __forceinline__ float fast_tanh(float x) {
   float e, r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * 2.8853900817779268f));   // exp(2x) = 2^(2x log2 e)
@@ -125,9 +97,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -135,30 +104,10 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-// arrive on the same-named barrier of CTA `rank` of this cluster.  Default semantics (release at CTA scope), as CUTLASS's
-// ClusterBarrier::arrive does: the arrival only hands TMEM back to the MMA warp, which tcgen05.fence::before_thread_sync has
-// already ordered; a `.release.cluster` arrive compiled to MEMBAR.ALL + ERRBAR per tile per epilogue warp of the follower
-// CTA (16 % of the GEMM's stall samples, profiles/r02_ncu_gemm_f16.txt).
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// Arrivals that only hand a TMEM buffer back (the reads were completed by tcgen05.wait::ld and ordered by
-// tcgen05.fence::before_thread_sync) need no memory ordering at all: relaxed, so that no MEMBAR waits for unrelated
-// outstanding loads of the arriving warp.
-__device__ __forceinline__ void mbar_arrive_relaxed(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.relaxed.cta.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote_relaxed(uint64_t* bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
 // Spin on a phase parity.  A deadlocked pipeline would otherwise hang the GPU until the watchdog kills the box, so
 // after 2^28 failed probes (each try_wait suspends the thread for a hardware-defined slice: seconds in total) the kernel
-// traps instead.  The loop body is the probe, one add and one compare: spinning producer / issuer warps share their
-// scheduler's issue slots with the epilogue and softmax warps.
+// traps instead.  The loop body is the probe, one add and one compare: a spinning producer warp shares its scheduler's
+// issue slots with the consumer warps.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
   uint32_t done = 0;
@@ -173,35 +122,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (done) break;
     if (it == (1u << 28)) __trap();
   }
-}
-
-// Non-blocking probe of a phase parity (mbarrier.test_wait never suspends the thread).
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(done)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return done != 0;
-}
-// Wait on two barriers whose probes are issued back to back, so their shared-memory round trips overlap
-// (a single probe costs a few hundred cycles while tcgen05.mma operand fetches saturate shared memory).
-__device__ __forceinline__ void mbar_wait2(uint64_t* a, uint32_t pa, uint64_t* b, uint32_t pb) {
-  const bool da = mbar_test(a, pa);
-  const bool db = mbar_test(b, pb);
-  if (!da) mbar_wait(a, pa);
-  if (!db) mbar_wait(b, pb);
-}
-__device__ __forceinline__ void mbar_wait3(uint64_t* a, uint32_t pa, uint64_t* b, uint32_t pb, uint64_t* c, uint32_t pc) {
-  const bool da = mbar_test(a, pa);
-  const bool db = mbar_test(b, pb);
-  const bool dc = mbar_test(c, pc);
-  if (!da) mbar_wait(a, pa);
-  if (!db) mbar_wait(b, pb);
-  if (!dc) mbar_wait(c, pc);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -222,186 +142,74 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
+// ------------------------------------------------------------------------------------------
+// warp-level tensor-core MMA (fp32 accumulate) and shared-memory fragment loads
+// ------------------------------------------------------------------------------------------
+// c[16x8] += a[16x8] . b[8x8], tf32 operands given as fp32 bit patterns (the tensor core ignores the low 13 bits)
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// TMA store smem -> global (bulk async-group completion), clipped at the tensor bounds
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+// c[16x8] += a[16x16] . b[16x8], fp16 operands (packed pairs)
+__device__ __forceinline__ void mma_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// four 8x8 fp16 matrices; lane l gives the shared-memory address of row l % 8 of matrix l / 8
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+// same, each matrix transposed on the way (rows in shared memory become columns of the fragment)
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+
+// ------------------------------------------------------------------------------------------
+// wgmma (sm_90a): warpgroup MMA on shared-memory descriptors, fp16 operands, fp32 accumulators in registers
+// ------------------------------------------------------------------------------------------
+// SWIZZLE_128B shared-memory matrix descriptor: start address, leading / stride byte offsets (16-byte units), layout 1
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-// 2-SM flavour: executed by both CTAs of a pair; the transaction bytes are credited to the
-// barrier of the even CTA (clear the peer bit, bit 24, of the shared::cluster address).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across the asynchronous MMA
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x N] += A[64 x 16] . B[16 x N]; TA / TB = 1: the operand is MN-major in shared memory (transposed)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %66, %67;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_3d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %34, %35;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
       : "memory");
-}
-
-// ------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads
-// ------------------------------------------------------------------------------------------
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], tf32 inputs, fp32 accumulate.  One thread issues.
-template <int CG>
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (CG == 1)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same, fp16 inputs (kind::f16), fp32 accumulate: UMMA_K = 16, twice the tf32 rate
-template <int CG>
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (CG == 1)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-template <int KIND, int CG>
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (KIND == 0) umma_tf32<CG>(d_tmem, adesc, bdesc, idesc, accumulate);
-  else                     umma_f16<CG>(d_tmem, adesc, bdesc, idesc, accumulate);
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-  else
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(smem_u32(bar)), "h"((uint16_t)0x3) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp receives lane (base+t).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M=128 rows = lanes, K along columns, one tf32 per
-// 32-bit column) is read from tensor memory, e.g. softmax probabilities written back over the scores
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// ------------------------------------------------------------------------------------------
-// descriptors
-// ------------------------------------------------------------------------------------------
-// SM100 shared-memory matrix descriptor, SWIZZLE_128B canonical layouts:
-//   bits [0,14)  start address >> 4      bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-//                (1 = SWIZZLE_128B_BASE32B: 32-byte chunks XOR (row % 4) -- the only layout
-//                 tcgen05 accepts for MN-major tf32 operands; TMA: SWIZZLE_128B_ATOM_32B)
-constexpr uint32_t kLayoutSw128 = 2, kLayoutSw128Base32 = 1;
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
-  return d;
-}
-// advance the start-address field of a descriptor by a byte offset (no carry out of the 14-bit
-// field as long as the operand stays inside the 227 KB window): one 64-bit add instead of
-// re-encoding -- the single MMA-issuing thread cannot hide ALU latency behind other warps
-__device__ __forceinline__ uint64_t desc_advance(uint64_t desc, uint32_t byte_off) { return desc + (uint64_t)(byte_off >> 4); }
-// instruction descriptor for kind::tf32, fp32 accumulate (upper 32 bits of the 64-bit idesc):
-//   [4,6) c_format=1(F32)  [7,10) a_format=2(TF32)  [10,13) b_format=2  [15] a_major  [16] b_major
-//   [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// instruction descriptor for kind::f16 with fp16 inputs, fp32 accumulate: a_format = b_format = 0 (F16)
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
 }
 // two fp32 -> packed fp16x2 (round to nearest), saturating at +-65504 instead of overflowing to inf
 __device__ __forceinline__ uint32_t pack_half2_sat(float a, float b) {

@@ -1,17 +1,18 @@
-// Persistent tensor-core GEMM for sm_100a: TMA -> 128B-swizzled smem ring -> tcgen05.mma (TMEM
-// accumulators, double buffered) -> fused epilogue.  Replaces every cuBLAS/cuDNN call the
-// reference issues for nn.Linear / Conv2d(k=s) / ConvTranspose2d(k=s) on the hot path
-// (reference enhancing/modules/stage1/layers.py:99-101,118-132,168-171,202-205) and their
-// dgrad / wgrad.
+// Persistent tensor-core GEMM for sm_90a: TMA -> 128B-swizzled smem ring (mbarrier full / empty pairs) ->
+// mma.sync on eight consumer warps (fp32 accumulators in registers) -> fused epilogue stored straight from
+// registers.  Replaces every cuBLAS/cuDNN call the reference issues for nn.Linear / Conv2d(k=s) /
+// ConvTranspose2d(k=s) on the hot path (reference enhancing/modules/stage1/layers.py:99-101,118-132,168-171,
+// 202-205) and their dgrad / wgrad.
 //
 //   C[M,N] = epilogue( alpha * sum_k A[m,k] * B[n,k] )              (per split z)
 //
 // Operand kinds (template KIND):
-//   0  fp32 storage, tcgen05 kind::tf32 (the tensor core keeps 10 mantissa bits: operands are rounded to
+//   0  fp32 storage, mma.sync m16n8k8 .tf32 (the tensor core keeps 10 mantissa bits: operands are rounded to
 //      nearest where they are produced).  With passes == 3 the contraction runs three times over
 //      (A_lo, B), (A, B_lo), (A, B) -- the error-compensated "3xTF32" product (lo = x - trunc_tf32(x),
 //      written by split_tf32_lo): fp32-grade results for the parity mode, at a third of the rate.
-//   1  fp16 storage, tcgen05 kind::f16, fp32 accumulate: the same 11-bit significand as tf32 at twice
+//   1  fp16 storage, wgmma m64nNk16 .f16 straight from the swizzled tiles (either major: wgmma transposes fp16
+//      operands itself), fp32 accumulate: the same 11-bit significand as tf32 at twice
 //      the tensor rate and half the operand bytes; gradients travel scaled by a power of two (alpha
 //      undoes it), so fp16's narrower exponent range is never the limit.
 // Output: fp32 (optionally tf32-rounded) or, with OUT16, fp16 (saturating).
@@ -23,10 +24,13 @@
 //   b_major = 1 : B is [K_total, N]  row-major                 (dgrad reads W, wgrad reads X)
 // Split-K: split z contracts rows/cols [z*K, (z+1)*K) and writes C + z*c_split_stride.
 //
-// Warp roles (320 threads): warp 0 = TMA producer, warp 1 = MMA issuer + TMEM owner,
-// warps 2..9 = epilogue (TMEM lane quarter = warp % 4; the two warps of a quarter take alternate
-// 32-column chunks so that one warp's TMEM-load / TMA latencies hide behind the other's math).  CG = 2 pairs two CTAs on one
-// 256 x BN tile (tcgen05 cta_group::2): each CTA stages its 128 rows of A and half of B.
+// Why the tf32 kinds use mma.sync: Hopper's wgmma reads tf32 operands from shared memory in K-major form only, and the
+// dgrad / wgrad products of the tf32 and parity data paths read MN-major operands.  Their mma.sync fragments are gathered
+// by the consumer warps themselves (scalar loads from the swizzled tiles), behind the same TMA ring and epilogue.
+//
+// Warp roles (288 threads): warps 0..7 consume, warp 8 is the TMA producer.  fp16: warpgroup w (warps 4w..4w+3) owns
+// rows 64w .. 64w+63 of the 128 x BN tile (warp 4w+i: rows 64w+16i .. +15); tf32: warp w owns rows 32*(w%4) .. +31
+// and half of the BN columns.
 #include "common.cuh"
 
 #include <mutex>
@@ -36,378 +40,283 @@ namespace b200 {
 
 struct GemmParams {
   int M, N, K;                 // output rows / cols, contraction length per split
-  int num_m_blocks;            // ceil(M / (128*CG)) cluster tiles along M
+  int num_m_blocks;            // ceil(M / 128)
   int num_n_blocks;            // ceil(N / BN)
   int num_splits;
-  int k_blocks;                // ceil(K / 32)
+  int k_blocks;                // ceil(K / BK)
   void* C;                     // fp32 or (OUT16) fp16
   long long ldc, c_split_stride;
   const float* alpha_ptr;      // device scalar multiplied into the accumulators (null = 1): undoes gradient scaling
   int passes;                  // 1, or 3 for the 3xTF32 split-operand product (KIND 0 only)
   const float* bias;           // [N] or null
-  const float* res;            // residual added in the epilogue through direct loads (row % res_row_mod), or null
+  const float* res;            // residual row (row % res_row_mod) added in the epilogue, or null
   long long ldres;
-  int res_row_mod;             // >0: residual row = row % res_row_mod (positional table)
-  int in_mode;                 // 0 none, 1: + tile of tmIn (residual), 2: * (1 - tile^2) (tanh backward)
+  int res_row_mod;
+  const void* in;              // in_mode 1: fp32 residual [M, ldin]; in_mode 2: tanh' input, output dtype [M, ldin]
+  long long ldin;
+  int in_mode;                 // 0 none, 1: + in (residual), 2: * (1 - in^2) (tanh backward)
   int act;                     // 0 none, 1 tanh
   int round_out;               // 1: round the stored value to tf32 (it only feeds another GEMM)
-  float* colsum_part;          // null, or [ceil(M/32)][N]: column sums of every 32-row group of the stored C
+  float* colsum_part;          // null, or [ceil(M/16)][N]: column sums of every 16-row group of the stored C
 };
 
 constexpr int kBM = 128;
-constexpr int kGemmThreads = 320;   // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
+constexpr int kConsumerWarps = 8;
+constexpr int kGemmThreads = 32 * (kConsumerWarps + 1);
 
 // per operand kind: a k-block is one 128-byte swizzle row of the operand's element type
 template <int KIND> struct Elem;
-template <> struct Elem<0> { static constexpr int BYTES = 4, BK = 32, MN_ATOM = 32, UMMA_K = 8, MN_SBO = 512;  static constexpr uint32_t MN_LAYOUT = kLayoutSw128Base32; };
-template <> struct Elem<1> { static constexpr int BYTES = 2, BK = 64, MN_ATOM = 64, UMMA_K = 16, MN_SBO = 1024; static constexpr uint32_t MN_LAYOUT = kLayoutSw128; };
+template <> struct Elem<0> { static constexpr int BYTES = 4, BK = 32, ATOM = 32, MMA_K = 8; };
+template <> struct Elem<1> { static constexpr int BYTES = 2, BK = 64, ATOM = 64, MMA_K = 16; };
 
-template <int BN, int CG>
+template <int BN>
 struct GemmCfg {
-  static constexpr int BN_CTA = BN / CG;
   static constexpr int A_BYTES = kBM * 128;       // 128 rows (or k-rows x atoms) of 128 bytes, either kind
-  static constexpr int B_BYTES = BN_CTA * 128;
+  static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGING_BYTES = 8 * 8192;      // per epilogue warp: out[4 KB] + in[4 KB]
-  static constexpr int MAX_SMEM = 232448;             // 227 KB opt-in limit
-  static constexpr int RING_BUDGET = MAX_SMEM - STAGING_BYTES - 1024 - 512;
+  static constexpr int MAX_SMEM = 232448;         // 227 KB opt-in limit
+  static constexpr int RING_BUDGET = MAX_SMEM - 1024 - 256;
   static constexpr int STAGES = (RING_BUDGET / STAGE_BYTES) > 8 ? 8 : (RING_BUDGET / STAGE_BYTES);
-  static constexpr int ACC_STRIDE = BN <= 64 ? 64 : (BN <= 128 ? 128 : 256);
-  static constexpr int TMEM_COLS = 2 * ACC_STRIDE;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 512 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-template <int KIND, int BN, int CG, int AMAJ, int BMAJ, int OUT16>
+// Byte offset of element (mn, k) of a stage tile, as TMA wrote it with SWIZZLE_128B (the tile base is 1024-aligned, so
+// the swizzle phase is the 128-byte row index mod 8).
+//   K-major : [mn][128 B of k]
+//   MN-major: [mn / ATOM][BK k-rows][128 B of mn]
+template <int KIND, int MAJ>
+__device__ __forceinline__ uint32_t tile_off(int mn, int k) {
+  using El = Elem<KIND>;
+  if constexpr (MAJ == 0) {
+    const uint32_t b = (uint32_t)k * El::BYTES;
+    return (uint32_t)mn * 128u + ((((b >> 4) ^ (uint32_t)mn) & 7u) << 4) + (b & 15u);
+  } else {
+    const uint32_t b = (uint32_t)(mn % El::ATOM) * El::BYTES;
+    return (uint32_t)(mn / El::ATOM) * (El::BK * 128u) + (uint32_t)k * 128u + ((((b >> 4) ^ (uint32_t)k) & 7u) << 4) + (b & 15u);
+  }
+}
+
+// P3: the 3xTF32 product (KIND 0, passes == 3), with per-k-block promotion of the partial sums
+template <int KIND, int BN, int AMAJ, int BMAJ, int OUT16, int P3>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmIn,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
-  using Cfg = GemmCfg<BN, CG>;
+  using Cfg = GemmCfg<BN>;
   using El = Elem<KIND>;
   constexpr int kBK = El::BK;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int WN = BN / 2;          // columns per consumer warp
+  constexpr int NT = WN / 8;          // n8 tiles per consumer warp
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* full_bar = bars;                    // [STAGES]
-  uint64_t* empty_bar = bars + STAGES;          // [STAGES]
-  uint64_t* tmem_full = bars + 2 * STAGES;      // [2]
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2; // [2]
-  uint64_t* in_full_all = bars + 2 * STAGES + 4;  // [8 epilogue warps]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 12);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);   // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                               // [STAGES]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const bool leader = cta_rank == 0;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
-    if (p.in_mode) tma_prefetch_desc(&tmIn);
-    for (int i = 0; i < 8; ++i) mbar_init(&in_full_all[i], 1);
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);    // the leader's producer arrives once, expecting the bytes of the whole pair
-      mbar_init(&empty_bar[s], 1);   // one tcgen05.commit
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 8 * CG);  // one arrive per epilogue warp of every CTA in the pair
+      mbar_init(&full_bar[s], 1);                  // the producer's expect_tx arrival
+      mbar_init(&empty_bar[s], kConsumerWarps);    // one arrival per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<CG>(tmem_slot, Cfg::TMEM_COLS);
-  tcgen05_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
   const int tiles_per_split = p.num_m_blocks * p.num_n_blocks;
   const int total_tiles = tiles_per_split * p.num_splits;
-  const int cluster_id = blockIdx.x / CG;
-  const int num_clusters = gridDim.x / CG;
+  const int kb_total = p.k_blocks * p.passes;
 
-  if (warp == 0) {
-    // ---------------------------------------------------------------- TMA producer (warp-uniform loop, one lane issues)
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-      const int z = t / tiles_per_split;
-      const int r = t - z * tiles_per_split;
-      const int mb = r / p.num_n_blocks, nb = r - mb * p.num_n_blocks;
-      const int m0 = (mb * CG + (int)cta_rank) * kBM;
-      const int n0 = nb * BN + (int)cta_rank * Cfg::BN_CTA;
-      const int kbase = z * p.K;
-      for (int pass = 0; pass < p.passes; ++pass) {
-        // 3xTF32: (A_lo, B) then (A, B_lo) then (A, B) -- small terms first; a single pass uses (A, B)
-        const CUtensorMap* mapA = (p.passes == 3 && pass == 0) ? &tmA2 : &tmA;
-        const CUtensorMap* mapB = (p.passes == 3 && pass == 1) ? &tmB2 : &tmB;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (elect_one()) {
+  if (warp == kConsumerWarps) {
+    // ---------------------------------------------------------------- TMA producer (one lane)
+    if (lane == 0) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmB);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        const int z = t / tiles_per_split;
+        const int r = t - z * tiles_per_split;
+        const int mb = r / p.num_n_blocks, nb = r - mb * p.num_n_blocks;
+        const int m0 = mb * kBM, n0 = nb * BN;
+        const int kbase = z * p.K;
+        for (int pass = 0; pass < p.passes; ++pass) {
+          // 3xTF32: (A_lo, B) then (A, B_lo) then (A, B) -- small terms first; a single pass uses (A, B)
+          const CUtensorMap* mapA = (p.passes == 3 && pass == 0) ? &tmA2 : &tmA;
+          const CUtensorMap* mapB = (p.passes == 3 && pass == 1) ? &tmB2 : &tmB;
+          for (int kb = 0; kb < p.k_blocks; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
             uint8_t* sb = sa + Cfg::A_BYTES;
             const int k0 = kbase + kb * kBK;
-            if constexpr (CG == 1) {
-              mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-              if constexpr (AMAJ == 0) tma_load_2d(sa, mapA, &full_bar[stage], k0, m0);
-              else                     tma_load_3d(sa, mapA, &full_bar[stage], 0, k0, m0 / El::MN_ATOM);
-              if constexpr (BMAJ == 0) tma_load_2d(sb, mapB, &full_bar[stage], k0, n0);
-              else                     tma_load_3d(sb, mapB, &full_bar[stage], 0, k0, n0 / El::MN_ATOM);
-            } else {
-              // Only the leader arrives (expecting both CTAs' bytes).  The follower's TMA credits
-              // the leader's barrier directly; it may land before the leader's expect_tx of the
-              // same phase (tx-count goes transiently negative), which is legal: the phase cannot
-              // complete before the leader's single pending arrival.
-              if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-              if constexpr (AMAJ == 0) tma_load_2d_2sm(sa, mapA, &full_bar[stage], k0, m0);
-              else                     tma_load_3d_2sm(sa, mapA, &full_bar[stage], 0, k0, m0 / El::MN_ATOM);
-              if constexpr (BMAJ == 0) tma_load_2d_2sm(sb, mapB, &full_bar[stage], k0, n0);
-              else                     tma_load_3d_2sm(sb, mapB, &full_bar[stage], 0, k0, n0 / El::MN_ATOM);
-            }
+            mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+            if constexpr (AMAJ == 0) tma_load_2d(sa, mapA, &full_bar[stage], k0, m0);
+            else                     tma_load_3d(sa, mapA, &full_bar[stage], 0, k0, m0 / El::ATOM);
+            if constexpr (BMAJ == 0) tma_load_2d(sb, mapB, &full_bar[stage], k0, n0);
+            else                     tma_load_3d(sb, mapB, &full_bar[stage], 0, k0, n0 / El::ATOM);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer (warp-uniform loop, one lane issues)
-    if (leader) {
-      constexpr uint32_t idesc = KIND == 0 ? make_idesc_tf32(kBM * CG, BN, AMAJ, BMAJ) : make_idesc_f16(kBM * CG, BN, AMAJ, BMAJ);
-      // K-major (SWIZZLE_128B): 8-row groups 1024 B apart (SBO), LBO unused; one UMMA_K step = 32 bytes.
-      // MN-major: smem holds [mn atom][BK k-rows][128 B]; atoms BK*128 B apart (LBO).
-      //   tf32: SWIZZLE_128B_BASE32B (mandatory for 32-bit MN-major), 4-k-row swizzle groups 512 B apart (SBO)
-      //   f16 : SWIZZLE_128B, 8-k-row groups 1024 B apart (SBO)
-      // one UMMA_K step = UMMA_K k-rows of 128 B.
-      constexpr uint32_t MN_LBO = kBK * 128;
-      constexpr uint32_t A_LBO = AMAJ ? MN_LBO : 16, B_LBO = BMAJ ? MN_LBO : 16;
-      constexpr uint32_t A_SBO = AMAJ ? El::MN_SBO : 1024, B_SBO = BMAJ ? El::MN_SBO : 1024;
-      constexpr uint32_t A_LAY = AMAJ ? El::MN_LAYOUT : kLayoutSw128, B_LAY = BMAJ ? El::MN_LAYOUT : kLayoutSw128;
-      constexpr uint32_t A_KSTEP = AMAJ ? El::UMMA_K * 128 : 32, B_KSTEP = BMAJ ? El::UMMA_K * 128 : 32;
-      const uint64_t a_desc0 = make_smem_desc(smem_u32(smem), A_LBO, A_SBO, A_LAY);
-      const uint64_t b_desc0 = make_smem_desc(smem_u32(smem) + Cfg::A_BYTES, B_LBO, B_SBO, B_LAY);
-      const int kb_total = p.k_blocks * p.passes;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int t = cluster_id; t < total_tiles; t += num_clusters, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::ACC_STRIDE;
-        for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          if (elect_one()) {
-            const uint64_t ad = desc_advance(a_desc0, stage * Cfg::STAGE_BYTES);
-            const uint64_t bd = desc_advance(b_desc0, stage * Cfg::STAGE_BYTES);
-#pragma unroll
-            for (int k = 0; k < kBK / El::UMMA_K; ++k)
-              umma_ss<KIND, CG>(d_tmem, desc_advance(ad, k * A_KSTEP), desc_advance(bd, k * B_KSTEP), idesc, (kb | k) != 0);
-            umma_commit<CG>(&empty_bar[stage]);  // frees the slot in both CTAs once the MMAs retire
-            if (kb == kb_total - 1) umma_commit<CG>(&tmem_full[acc]);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- epilogue warps
-    // Each warp owns 32 rows of the tile (TMEM lane quarter q) and every other column chunk (32 fp32 columns,
-    // or 64 columns when the output is fp16: either way one 32-row x 128-byte box).
-    // Per chunk: tcgen05.ld -> registers -> fused math -> 128B-swizzled smem box -> TMA store (fully
-    // coalesced, clipped at the matrix edge).  Residual / tanh' inputs arrive the same way through
-    // TMA loads issued one chunk ahead.
-    constexpr int CW = OUT16 ? 64 : 32;      // chunk width in columns
-    const int q = warp & 3;  // TMEM lane quarter this warp may touch
-    const int ew = warp - 2;
-    const int ehalf = ew >> 2;
-    uint8_t* const box0 = staging + ew * 8192;
-    uint8_t* in_buf = box0 + 4096;
-    uint64_t* in_full = in_full_all + ew;
-    const uint32_t swz = lane & 7;
-    const bool tma_in = p.in_mode != 0;
-    const float alpha = p.alpha_ptr ? __ldg(p.alpha_ptr) : 1.f;
-    uint32_t in_cnt = 0, out_cnt = 0;
-    constexpr int NCHUNK = BN / CW;
-    int it = 0;
-    for (int t = cluster_id; t < total_tiles; t += num_clusters, ++it) {
-      const int z = t / tiles_per_split;
-      const int r = t - z * tiles_per_split;
-      const int mb = r / p.num_n_blocks, nb = r - mb * p.num_n_blocks;
-      const int row0 = (mb * CG + (int)cta_rank) * kBM + q * 32;
-      const int row = row0 + lane;
-      const int n0 = nb * BN;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      if (tma_in && ehalf < NCHUNK && lane == 0) {   // this warp's first input chunk of the tile (buffer free since the last tile)
-        mbar_arrive_expect_tx(in_full, 4096);
-        tma_load_2d(in_buf, &tmIn, in_full, n0 + ehalf * CW, row0);
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_fence_after();
-      const float* rrow = nullptr;
-      if (p.res && row < p.M) rrow = p.res + (long long)(p.res_row_mod > 0 ? row % p.res_row_mod : row) * p.ldres;
-#pragma unroll 1
-      for (int c = ehalf; c < NCHUNK; c += 2) {
-        const int col0 = n0 + c * CW;
-        uint32_t v[CW];
-        {
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * Cfg::ACC_STRIDE + c * CW;
-          tmem_ld_32x32(taddr, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-          if constexpr (CW == 64) tmem_ld_32x32(taddr + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-        }
-        uint4 a[8];     // the input box row of this lane: 32 fp32 (OUT16 == 0) or 64 fp16 (OUT16 == 1)
-        if (tma_in) {
-          mbar_wait(in_full, in_cnt & 1);
-          ++in_cnt;
-          const uint8_t* inb = in_buf + lane * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) a[j] = *reinterpret_cast<const uint4*>(inb + ((j ^ swz) << 4));
-        }
-        tmem_ld_wait();
-        if (tma_in) {   // placed after the TMEM wait so that the stall on the loads below is already paid for
-          // The refill below overwrites in_buf through the async proxy, so every lane's loads of this chunk must
-          // have *completed*, not merely issued: while tcgen05.mma operand fetches saturate shared memory a
-          // load can stay in flight longer than a TMA round trip (seen as one stale 16-byte group per few
-          // thousand tiles).  The two complementary ballots consume a loaded register of every 16-byte group of
-          // every lane (a real instruction per lane, so the scoreboard wait cannot be scheduled past it) and
-          // together always report all 32 lanes -- whatever the tile holds, NaN patterns included -- so the
-          // refill is data-ordered but never skipped.
-          uint32_t bits = 0;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) bits |= a[j].x;
-          const uint32_t landed = __ballot_sync(0xffffffffu, bits != 0x7fc0deadu) | __ballot_sync(0xffffffffu, bits == 0x7fc0deadu);
-          if (lane == 0 && c + 2 < NCHUNK && landed != 0u) {
-            mbar_arrive_expect_tx(in_full, 4096);
-            tma_load_2d(in_buf, &tmIn, in_full, col0 + 2 * CW, row0);
-          }
-        }
-        // Store staging: without a TMA-fed epilogue input the input box is free, so the warp alternates between two
-        // store boxes and only waits for the store *before* the previous one (its smem reads overlap this chunk's
-        // TMEM load and math); with an input box there is a single store box and the wait is for the previous store.
-        uint8_t* const out_buf = (tma_in || !(out_cnt & 1)) ? box0 : in_buf;
-        ++out_cnt;
-        if (lane == 0) { if (tma_in) bulk_wait_group_read<0>(); else bulk_wait_group_read<1>(); }
-        __syncwarp();
-        uint8_t* outb = out_buf + lane * 128;
-        if constexpr (OUT16 == 0) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 o = make_float4(__uint_as_float(v[4 * j]) * alpha, __uint_as_float(v[4 * j + 1]) * alpha,
-                                   __uint_as_float(v[4 * j + 2]) * alpha, __uint_as_float(v[4 * j + 3]) * alpha);
-            const int col = col0 + 4 * j;
-            if (p.bias && col < p.N) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-              o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-            }
-            if (p.act == 1) { o.x = fast_tanh(o.x); o.y = fast_tanh(o.y); o.z = fast_tanh(o.z); o.w = fast_tanh(o.w); }
-            if (tma_in) {
-              const float4 ai = make_float4(__uint_as_float(a[j].x), __uint_as_float(a[j].y), __uint_as_float(a[j].z), __uint_as_float(a[j].w));
-              if (p.in_mode == 2) {
-                o.x *= 1.f - ai.x * ai.x; o.y *= 1.f - ai.y * ai.y; o.z *= 1.f - ai.z * ai.z; o.w *= 1.f - ai.w * ai.w;
-              } else {
-                o.x += ai.x; o.y += ai.y; o.z += ai.z; o.w += ai.w;
-              }
-            }
-            if (rrow && col < p.N) {
-              const float4 rr = __ldg(reinterpret_cast<const float4*>(rrow + col));
-              o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w;
-            }
-            if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-            *reinterpret_cast<float4*>(outb + ((j ^ swz) << 4)) = o;
-          }
-        } else {
-          // fp16 output: 8 columns per 16-byte group; optional bias -> tanh -> * (1 - aux^2) with an fp16 aux box
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = __uint_as_float(v[8 * j + e]) * alpha;
-            const int col = col0 + 8 * j;
-            if (p.bias && col < p.N) {
-              const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-              const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
-              o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w; o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-            }
-            if (p.act == 1) {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) o[e] = fast_tanh(o[e]);
-            }
-            if (tma_in) {   // in_mode 2 is the only fp16 input: tanh' from the saved fp16 activation
-              const uint32_t w[4] = {a[j].x, a[j].y, a[j].z, a[j].w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 t2 = __half22float2(*reinterpret_cast<const __half2*>(&w[e]));
-                o[2 * e] *= 1.f - t2.x * t2.x;
-                o[2 * e + 1] *= 1.f - t2.y * t2.y;
-              }
-            }
-            uint4 pk;
-            pk.x = pack_half2_sat(o[0], o[1]); pk.y = pack_half2_sat(o[2], o[3]);
-            pk.z = pack_half2_sat(o[4], o[5]); pk.w = pack_half2_sat(o[6], o[7]);
-            *reinterpret_cast<uint4*>(outb + ((j ^ swz) << 4)) = pk;
-          }
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          if (col0 < p.N && row0 < p.M) tma_store_3d(&tmC, out_buf, col0, row0, z);
-          bulk_commit_group();
-        }
-        if (p.colsum_part) {
-          // bias gradient for free: each lane sums its column(s) of the box just staged (rows past M hold
-          // epilogue constants and are skipped); the row-group partials are reduced by a colsum launch
-          const int rmax = p.M - row0;
-          const uint8_t* colp = out_buf + ((lane & 3) << 2);
-          const uint32_t cj = lane >> 2;
-          float cs0 = 0.f, cs1 = 0.f;
-#pragma unroll 1
-          for (int rb = 0; rb < 32; rb += 8) {       // 8 rows = one swizzle period; kept rolled so the 32 addresses are not hoisted
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              if (rb + k < rmax) {
-                const uint32_t wv = *reinterpret_cast<const uint32_t*>(colp + (rb + k) * 128 + ((cj ^ k) << 4));
-                if constexpr (OUT16 == 0) {
-                  if (k & 1) cs1 += __uint_as_float(wv); else cs0 += __uint_as_float(wv);
-                } else {
-                  const float2 h2 = __half22float2(*reinterpret_cast<const __half2*>(&wv));
-                  cs0 += h2.x; cs1 += h2.y;
-                }
-              }
-            }
-          }
-          if (row0 < p.M) {
-            float* dst = p.colsum_part + (size_t)(row0 >> 5) * p.N;
-            if constexpr (OUT16 == 0) {
-              if (col0 + lane < p.N) dst[col0 + lane] = cs0 + cs1;
-            } else {
-              if (col0 + 2 * lane < p.N) { dst[col0 + 2 * lane] = cs0; dst[col0 + 2 * lane + 1] = cs1; }
-            }
-          }
-        }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CG == 1 || leader) mbar_arrive_relaxed(&tmem_empty[acc]);
-        else                   mbar_arrive_remote_relaxed(&tmem_empty[acc], 0);
-      }
-    }
-    if (lane == 0) bulk_wait_group_read<0>();   // smem must outlive the last stores' reads
+    return;
   }
 
-  // ------------------------------------------------------------------ teardown
-  tcgen05_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<CG>(tmem_base, Cfg::TMEM_COLS);
+  // ------------------------------------------------------------------ consumers: main loop + epilogue
+  const int wm = warp & 3, wn = warp >> 2;
+  const int g = lane >> 2, tq = lane & 3;
+  const float alpha = p.alpha_ptr ? __ldg(p.alpha_ptr) : 1.f;
+  const uint32_t smem_base = smem_u32(smem);
+  // accumulator shape per warp: MT m16 tiles x NTW n8 tiles, each in the mma.sync / wgmma fragment layout
+  // (c0, c1: row g, columns 2tq, 2tq+1; c2, c3: row g + 8)
+  constexpr bool WG = KIND == 1;
+  constexpr int MT = WG ? 1 : 2;
+  constexpr int NTW = WG ? BN / 8 : NT;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    const int z = t / tiles_per_split;
+    const int r = t - z * tiles_per_split;
+    const int mb = r / p.num_n_blocks, nb = r - mb * p.num_n_blocks;
+    float acc[MT][NTW][4];
+#pragma unroll
+    for (int i = 0; i < MT; ++i)
+#pragma unroll
+      for (int j = 0; j < NTW; ++j) acc[i][j][0] = acc[i][j][1] = acc[i][j][2] = acc[i][j][3] = 0.f;
+    // 3xTF32: the tensor core's internal fp32 accumulation truncates, which over a long contraction costs the product
+    // its fp32 grade.  Each k-block is therefore summed into a zeroed partial and promoted into acc with a rounded FADD.
+    constexpr bool promote = P3 != 0;
+    float part[MT][NTW][4];
+#pragma unroll
+    for (int i = 0; i < MT; ++i)
+#pragma unroll
+      for (int j = 0; j < NTW; ++j) part[i][j][0] = part[i][j][1] = part[i][j][2] = part[i][j][3] = 0.f;
+
+    for (int kb = 0; kb < kb_total; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+      const uint8_t* sb = sa + Cfg::A_BYTES;
+      if constexpr (KIND == 0) {
+#pragma unroll
+        for (int ks = 0; ks < kBK / El::MMA_K; ++ks) {
+          const int k0 = ks * El::MMA_K;
+          uint32_t af[2][4], bf[NT][2];
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            const int m = wm * 32 + mt * 16 + g;
+            af[mt][0] = *reinterpret_cast<const uint32_t*>(sa + tile_off<0, AMAJ>(m, k0 + tq));
+            af[mt][1] = *reinterpret_cast<const uint32_t*>(sa + tile_off<0, AMAJ>(m + 8, k0 + tq));
+            af[mt][2] = *reinterpret_cast<const uint32_t*>(sa + tile_off<0, AMAJ>(m, k0 + tq + 4));
+            af[mt][3] = *reinterpret_cast<const uint32_t*>(sa + tile_off<0, AMAJ>(m + 8, k0 + tq + 4));
+          }
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) {
+            const int n = wn * WN + nt * 8 + g;
+            bf[nt][0] = *reinterpret_cast<const uint32_t*>(sb + tile_off<0, BMAJ>(n, k0 + tq));
+            bf[nt][1] = *reinterpret_cast<const uint32_t*>(sb + tile_off<0, BMAJ>(n, k0 + tq + 4));
+          }
+          if constexpr (promote) {
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+              for (int nt = 0; nt < NT; ++nt) mma_tf32(part[mt][nt], af[mt], bf[nt][0], bf[nt][1]);
+          } else {
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+              for (int nt = 0; nt < NT; ++nt) mma_tf32(acc[mt][nt], af[mt], bf[nt][0], bf[nt][1]);
+          }
+        }
+      } else {
+        // one warpgroup-wide MMA per 16-deep k step: A = this warpgroup's 64 rows, B = the whole BN-column tile.
+        // K-major: 8-row groups 1024 B apart (SBO), a k step is 32 B along the row.  MN-major: 64-element atoms
+        // kBK*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO), a k step is 16 k-rows = 2048 B.
+        const int wg = warp >> 2;
+        const uint32_t sa_u = smem_base + stage * Cfg::STAGE_BYTES, sb_u = sa_u + Cfg::A_BYTES;
+        const uint32_t a0 = sa_u + wg * (AMAJ ? kBK * 128 : 64 * 128);
+        float (&d)[BN / 2] = *reinterpret_cast<float(*)[BN / 2]>(&acc[0][0][0]);
+        wgmma_fence_regs(d);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kBK / El::MMA_K; ++ks) {
+          const uint64_t ad = wgmma_desc_sw128(a0 + ks * (AMAJ ? 2048 : 32), kBK * 128, 1024);
+          const uint64_t bd = wgmma_desc_sw128(sb_u + ks * (BMAJ ? 2048 : 32), kBK * 128, 1024);
+          if constexpr (BN == 128) wgmma_m64n128k16_f16<AMAJ, BMAJ>(d, ad, bd);
+          else                     wgmma_m64n64k16_f16<AMAJ, BMAJ>(d, ad, bd);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(d);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      if constexpr (promote) {
+#pragma unroll
+        for (int i = 0; i < MT; ++i)
+#pragma unroll
+          for (int j = 0; j < NTW; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) { acc[i][j][e] += part[i][j][e]; part[i][j][e] = 0.f; }
+      }
+    }
+
+    // ---------------------------------------------------------------- epilogue (rows g, g + 8 of each m16 tile)
+    const long long zoff = (long long)z * p.c_split_stride;
+#pragma unroll
+    for (int nt = 0; nt < NTW; ++nt) {
+      const int col = nb * BN + (WG ? 0 : wn * WN) + nt * 8 + 2 * tq;
+      const bool col_ok = col < p.N;     // N is even, so col + 1 < N as well
+      float2 bias2 = make_float2(0.f, 0.f);
+      if (p.bias && col_ok) bias2 = *reinterpret_cast<const float2*>(p.bias + col);
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+        const int row16 = mb * kBM + (WG ? warp * 16 : wm * 32 + mt * 16);
+        float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {    // row half: g, g + 8
+          const int row = row16 + g + h * 8;
+          float o0 = acc[mt][nt][h * 2] * alpha + bias2.x;
+          float o1 = acc[mt][nt][h * 2 + 1] * alpha + bias2.y;
+          if (row >= p.M || !col_ok) continue;
+          if (p.act == 1) { o0 = fast_tanh(o0); o1 = fast_tanh(o1); }
+          if (p.in_mode == 1) {
+            const float2 a = *reinterpret_cast<const float2*>(static_cast<const float*>(p.in) + (long long)row * p.ldin + col);
+            o0 += a.x; o1 += a.y;
+          } else if (p.in_mode == 2) {
+            float2 a;
+            if constexpr (OUT16) a = __half22float2(*reinterpret_cast<const __half2*>(static_cast<const __half*>(p.in) + (long long)row * p.ldin + col));
+            else                 a = *reinterpret_cast<const float2*>(static_cast<const float*>(p.in) + (long long)row * p.ldin + col);
+            o0 *= 1.f - a.x * a.x; o1 *= 1.f - a.y * a.y;
+          }
+          if (p.res) {
+            const float2 rr = *reinterpret_cast<const float2*>(p.res + (long long)(row % p.res_row_mod) * p.ldres + col);
+            o0 += rr.x; o1 += rr.y;
+          }
+          if constexpr (OUT16) {
+            const uint32_t pk = pack_half2_sat(o0, o1);
+            *reinterpret_cast<uint32_t*>(static_cast<__half*>(p.C) + zoff + (long long)row * p.ldc + col) = pk;
+            const float2 st = __half22float2(*reinterpret_cast<const __half2*>(&pk));
+            cs0 += st.x; cs1 += st.y;
+          } else {
+            if (p.round_out) { o0 = round_tf32(o0); o1 = round_tf32(o1); }
+            *reinterpret_cast<float2*>(static_cast<float*>(p.C) + zoff + (long long)row * p.ldc + col) = make_float2(o0, o1);
+            cs0 += o0; cs1 += o1;
+          }
+        }
+        if (p.colsum_part) {
+          // bias gradient for free: the m16 tile's rows are one 16-row group of the partial-sum table
+#pragma unroll
+          for (int off = 4; off < 32; off <<= 1) {
+            cs0 += __shfl_xor_sync(0xffffffffu, cs0, off);
+            cs1 += __shfl_xor_sync(0xffffffffu, cs1, off);
+          }
+          if (g == 0 && col_ok && row16 < p.M)
+            *reinterpret_cast<float2*>(p.colsum_part + (size_t)(row16 >> 4) * p.N + col) = make_float2(cs0, cs1);
+        }
+      }
+    }
   }
 }
 
@@ -473,10 +382,9 @@ int make_tensor_map(CUtensorMap* out, const void* ptr, int elem_bytes, int rank,
   cuuint32_t bx[5], es[5];
   for (int i = 0; i < rank; ++i) { d[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) st[i] = strides_bytes[i];
-  static const CUtensorMapSwizzle kSwz[4] = {CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
-                                             CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_SWIZZLE_NONE};
+  static const CUtensorMapSwizzle kSwz[3] = {CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_SWIZZLE_NONE};
   CUresult r = enc(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank,
-                   const_cast<void*>(ptr), d, st, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, kSwz[swizzle & 3],
+                   const_cast<void*>(ptr), d, st, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, kSwz[swizzle < 0 || swizzle > 2 ? 2 : swizzle],
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return set_error(-4, "cuTensorMapEncodeTiled failed (%d) ptr=%p esz=%d rank=%d dims0=%llu box0=%u", (int)r, ptr, elem_bytes, rank,
@@ -501,73 +409,63 @@ static int make_operand_tmap(CUtensorMap* out, const void* ptr, int esz, long lo
   const unsigned long long dims[3] = {atom, (unsigned long long)rows, (unsigned long long)(cols / atom)};
   const unsigned long long strides[2] = {(unsigned long long)ld * esz, 128};
   const unsigned box[3] = {atom, atom, (unsigned)(box_mn / atom)};
-  return make_tensor_map(out, ptr, esz, 3, dims, strides, box, esz == 4 ? 1 : 0);
+  return make_tensor_map(out, ptr, esz, 3, dims, strides, box, 0);
 }
 
-struct GemmMaps { CUtensorMap a, b, c, in, a2, b2; };
+struct GemmMaps { CUtensorMap a, b, a2, b2; };
 
-template <int KIND, int BN, int CG, int AMAJ, int BMAJ, int OUT16>
+template <int KIND, int BN, int AMAJ, int BMAJ, int OUT16, int P3 = 0>
 static int launch_gemm(const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, CG>;
-  auto kern = gemm_tc_kernel<KIND, BN, CG, AMAJ, BMAJ, OUT16>;
+  using Cfg = GemmCfg<BN>;
+  auto kern = gemm_tc_kernel<KIND, BN, AMAJ, BMAJ, OUT16, P3>;
   B200_CONFIGURE_SMEM_ONCE(kern, Cfg::SMEM_BYTES);
   const int total = p.num_m_blocks * p.num_n_blocks * p.num_splits;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((num_sms() / CG) * CG);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  // persistent kernel: launch exactly as many clusters as can be co-resident (a CTA pair needs
-  // two free SMs of one TPC; fewer than num_sms/2 pairs may fit) so that no cluster waits for
-  // a second wave behind CTAs that never exit early
+  // persistent kernel: launch exactly as many CTAs as can be co-resident, so that none waits for a second wave behind
+  // CTAs that never exit early
   static PerDevice occ;
   const int dev = current_device();
   if (dev < 0 || dev >= kMaxDevices) return set_error(-2, "no current CUDA device");
   if (!occ.done[dev]) {
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) n = num_sms() / CG;
-    occ.value[dev] = n;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kGemmThreads, Cfg::SMEM_BYTES) != cudaSuccess || n <= 0) n = 1;
+    occ.value[dev] = n * num_sms();
     occ.done[dev] = true;
   }
-  int clusters = occ.value[dev] < total ? occ.value[dev] : total;
+  int ctas = occ.value[dev] < total ? occ.value[dev] : total;
   const int cap = sm_limit();          // optional cap (B200VQ_SM_LIMIT / b200vq_set_sm_limit): leave SMs to a concurrent NCCL kernel
-  if (cap > 0 && clusters * CG > cap) clusters = cap / CG > 0 ? cap / CG : 1;
-  cfg.gridDim = dim3(clusters * CG);
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm.a, tm.b, tm.c, tm.in, tm.a2, tm.b2, p));
-  count_launch();
+  if (cap > 0 && ctas > cap) ctas = cap;
+  kern<<<ctas, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tm.a, tm.b, tm.a2, tm.b2, p);
+  B200_LAUNCH_OK("gemm_tc_kernel");
   return 0;
 }
 
-template <int KIND, int BN, int CG>
+template <int KIND, int BN, int P3 = 0>
 static int dispatch_major(int am, int bm, int out16, const GemmMaps& tm, const GemmParams& p, cudaStream_t s) {
   if constexpr (KIND == 0) {
-    if (am == 0 && bm == 0) return launch_gemm<0, BN, CG, 0, 0, 0>(tm, p, s);
-    if (am == 0 && bm == 1) return launch_gemm<0, BN, CG, 0, 1, 0>(tm, p, s);
-    if (am == 1 && bm == 1) return launch_gemm<0, BN, CG, 1, 1, 0>(tm, p, s);
-    if (am == 1 && bm == 0) return launch_gemm<0, BN, CG, 1, 0, 0>(tm, p, s);
+    if (am == 0 && bm == 0) return launch_gemm<0, BN, 0, 0, 0, P3>(tm, p, s);
+    if (am == 0 && bm == 1) return launch_gemm<0, BN, 0, 1, 0, P3>(tm, p, s);
+    if (am == 1 && bm == 1) return launch_gemm<0, BN, 1, 1, 0, P3>(tm, p, s);
+    if (am == 1 && bm == 0) return launch_gemm<0, BN, 1, 0, 0, P3>(tm, p, s);
   } else {
     // the combinations the fp16 data path uses: forward x W^T and dgrad g W with fp32 or fp16 output; wgrad (fp32)
-    if (am == 0 && bm == 0) return out16 ? launch_gemm<1, BN, CG, 0, 0, 1>(tm, p, s) : launch_gemm<1, BN, CG, 0, 0, 0>(tm, p, s);
-    if (am == 0 && bm == 1) return out16 ? launch_gemm<1, BN, CG, 0, 1, 1>(tm, p, s) : launch_gemm<1, BN, CG, 0, 1, 0>(tm, p, s);
-    if (am == 1 && bm == 1 && !out16) return launch_gemm<1, BN, CG, 1, 1, 0>(tm, p, s);
+    if (am == 0 && bm == 0) return out16 ? launch_gemm<1, BN, 0, 0, 1>(tm, p, s) : launch_gemm<1, BN, 0, 0, 0>(tm, p, s);
+    if (am == 0 && bm == 1) return out16 ? launch_gemm<1, BN, 0, 1, 1>(tm, p, s) : launch_gemm<1, BN, 0, 1, 0>(tm, p, s);
+    if (am == 1 && bm == 1 && !out16) return launch_gemm<1, BN, 1, 1, 0>(tm, p, s);
   }
   return set_error(-1, "gemm: operand major (%d,%d) with out16=%d is not built for kind %d", am, bm, out16, KIND);
 }
 
 // kind 0: A/B fp32 (tf32 tensor cores; A_lo/B_lo non-null selects the 3-pass error-compensated product)
 // kind 1: A/B fp16
+// cta_group is accepted for ABI stability and ignored (one CTA per tile on sm_90a); bn <= 64 selects 64-column
+// tiles, anything else 128.  The 3xTF32 product always runs on 64-column tiles: its promoted partial sums double the
+// accumulator registers.
 static int gemm_launch(int kind, const void* A, long long lda, int a_major, const void* B, long long ldb, int b_major, void* C,
                        long long ldc, int out16, int M, int N, int K, int splits, long long c_split_stride, const float* bias,
                        const float* res, long long ldres, int res_row_mod, const void* aux, long long ldaux, float* colsum_part,
                        int act, int round_out, const float* alpha_ptr, const float* A_lo, const float* B_lo, int cta_group, int bn,
                        cudaStream_t stream) {
+  (void)cta_group;
   const int esz = kind == 0 ? 4 : 2;          // operand element bytes
   const int osz = out16 ? 2 : 4;              // output element bytes
   const int atom = 128 / esz;
@@ -584,79 +482,46 @@ static int gemm_launch(int kind, const void* A, long long lda, int a_major, cons
   B200_CHECK_ARG(!aux || ldaux * (out16 ? 2 : 4) % 16 == 0, "gemm: ldaux must give 16-byte rows");
   B200_CHECK_ARG(!out16 || (!res && splits == 1 && !round_out), "gemm: fp16 output takes no residual / split-K / tf32 rounding");
   B200_CHECK_ARG(!(A_lo || B_lo) || (kind == 0 && A_lo && B_lo), "gemm: the 3xTF32 product needs both A_lo and B_lo (fp32 operands)");
-  if (cta_group != 2) cta_group = 1;
-  if (bn <= 0) bn = N >= 256 ? 256 : (N > 128 ? (N <= 192 ? 192 : 256) : (N > 64 ? 128 : 64));
+  B200_CHECK_ARG(splits == 1 || c_split_stride % 4 == 0, "gemm: c_split_stride %% 4");
+  B200_CHECK_ARG(!(aux && res && res_row_mod == 0), "gemm: residual and tanh' inputs cannot be combined");
+  if (bn <= 0) bn = N > 64 ? 128 : 64;
   B200_CHECK_ARG(bn == 64 || bn == 128 || bn == 192 || bn == 256, "gemm: unsupported BN %d", bn);
-  if (kind == 1 && b_major == 1 && (bn / cta_group) % 64) bn = bn <= 128 ? 128 : 256;   // a CTA stages whole 64-column atoms of B
-  if (out16 && bn % 64) bn = 256;
+  bn = (bn <= 64 || A_lo) ? 64 : 128;
 
   GemmParams p;
   p.M = M; p.N = N; p.K = K;
-  p.num_m_blocks = (M + kBM * cta_group - 1) / (kBM * cta_group);
+  p.num_m_blocks = (M + kBM - 1) / kBM;
   p.num_n_blocks = (N + bn - 1) / bn;
   p.num_splits = splits;
   p.k_blocks = (K + atom - 1) / atom;
   p.C = C; p.ldc = ldc; p.c_split_stride = c_split_stride;
   p.alpha_ptr = alpha_ptr;
   p.passes = A_lo ? 3 : 1;
-  B200_CHECK_ARG(!(aux && res && res_row_mod == 0), "gemm: residual and tanh' inputs cannot be combined");
   p.bias = bias; p.act = act; p.round_out = round_out; p.colsum_part = colsum_part;
   p.res = (res && res_row_mod > 0) ? res : nullptr; p.ldres = ldres; p.res_row_mod = res_row_mod;
   p.in_mode = aux ? 2 : ((res && res_row_mod == 0) ? 1 : 0);
+  p.in = aux ? aux : static_cast<const void*>(res);
+  p.ldin = aux ? ldaux : ldres;
+  B200_CHECK_ARG(!p.in_mode || (reinterpret_cast<uintptr_t>(p.in) & 15) == 0, "gemm: epilogue input must be 16-byte aligned");
 
   GemmMaps tm;
-  {
-    const unsigned cw = out16 ? 64 : 32;      // columns per 128-byte store box
-    const unsigned long long dims[3] = {(unsigned long long)N, (unsigned long long)M, (unsigned long long)splits};
-    const unsigned long long strides[2] = {(unsigned long long)ldc * osz,
-                                           (unsigned long long)(splits > 1 ? c_split_stride : (long long)M * ldc) * osz};
-    const unsigned box[3] = {cw, 32, 1};
-    B200_CHECK_ARG(splits == 1 || c_split_stride % 4 == 0, "gemm: c_split_stride %% 4");
-    int rc0 = make_tensor_map(&tm.c, C, osz, 3, dims, strides, box, 0);
-    if (rc0) return rc0;
-    tm.in = tm.c;
-    if (p.in_mode) {
-      // residual: fp32 box of 32 columns; tanh' input: same element type and box as the output
-      const void* src = aux ? aux : static_cast<const void*>(res);
-      const long long ldin = aux ? ldaux : ldres;
-      const int isz = aux ? osz : 4;
-      B200_CHECK_ARG((reinterpret_cast<uintptr_t>(src) & 15) == 0, "gemm: epilogue input must be 16-byte aligned");
-      const unsigned long long d2[2] = {(unsigned long long)N, (unsigned long long)M};
-      const unsigned long long s2[1] = {(unsigned long long)ldin * isz};
-      const unsigned b2[2] = {128u / isz, 32};
-      rc0 = make_tensor_map(&tm.in, src, isz, 2, d2, s2, b2, 0);
-      if (rc0) return rc0;
-    }
-  }
   const int ktot = K * splits;
-  const int bn_cta = bn / cta_group;
   int rc;
   auto opmap = [&](CUtensorMap* out, const void* ptr, long long ld, int mn, int major, int box_mn) {
     return major == 0 ? make_operand_tmap(out, ptr, esz, ld, mn, ktot, 0, box_mn) : make_operand_tmap(out, ptr, esz, ld, ktot, mn, 1, box_mn);
   };
   if ((rc = opmap(&tm.a, A, lda, M, a_major, kBM))) return rc;
-  if ((rc = opmap(&tm.b, B, ldb, N, b_major, bn_cta))) return rc;
+  if ((rc = opmap(&tm.b, B, ldb, N, b_major, bn))) return rc;
   tm.a2 = tm.a; tm.b2 = tm.b;
   if (A_lo) {
     if ((rc = opmap(&tm.a2, A_lo, lda, M, a_major, kBM))) return rc;
-    if ((rc = opmap(&tm.b2, B_lo, ldb, N, b_major, bn_cta))) return rc;
+    if ((rc = opmap(&tm.b2, B_lo, ldb, N, b_major, bn))) return rc;
   }
-
-#define B200_GEMM_CASE(BN_)                                                                                        \
-  case BN_:                                                                                                        \
-    if (kind == 0)                                                                                                 \
-      return cta_group == 2 ? dispatch_major<0, BN_, 2>(a_major, b_major, 0, tm, p, stream)                        \
-                            : dispatch_major<0, BN_, 1>(a_major, b_major, 0, tm, p, stream);                       \
-    return cta_group == 2 ? dispatch_major<1, BN_, 2>(a_major, b_major, out16, tm, p, stream)                      \
-                          : dispatch_major<1, BN_, 1>(a_major, b_major, out16, tm, p, stream);
-  switch (bn) {
-    B200_GEMM_CASE(64)
-    B200_GEMM_CASE(128)
-    B200_GEMM_CASE(192)
-    B200_GEMM_CASE(256)
-  }
-#undef B200_GEMM_CASE
-  return set_error(-1, "gemm: unreachable");
+  if (A_lo) return dispatch_major<0, 64, 1>(a_major, b_major, 0, tm, p, stream);
+  if (bn == 64) return kind == 0 ? dispatch_major<0, 64>(a_major, b_major, 0, tm, p, stream)
+                                 : dispatch_major<1, 64>(a_major, b_major, out16, tm, p, stream);
+  return kind == 0 ? dispatch_major<0, 128>(a_major, b_major, 0, tm, p, stream)
+                   : dispatch_major<1, 128>(a_major, b_major, out16, tm, p, stream);
 }
 
 int gemm_tf32(const float* A, long long lda, int a_major, const float* B, long long ldb, int b_major, float* C,

@@ -1,4 +1,4 @@
-// The two native ops of the reference's loss stage (SURVEY.md section 8f-2), rebuilt for sm_100a behind the C ABI:
+// The two native ops of the reference's loss stage (SURVEY.md section 8f-2), rebuilt for sm_90a behind the C ABI:
 //   bias_act   -- reference enhancing/losses/op/fused_bias_act_kernel.cu (StyleGAN2 fused bias + leaky-ReLU + gain, and
 //                 its first/second derivative forms), called by losses/op/fused_act.py:62-91;
 //   upfirdn2d  -- reference enhancing/losses/op/upfirdn2d_kernel.cu (zero-insert upsample -> FIR -> decimate),

@@ -225,7 +225,7 @@ __global__ void colpart_reduce_kernel(const float* __restrict__ part, int nparts
 
 // part is [nparts][nacc][D] -> dgamma[D], dbeta[D] (, dxsum[D]).  A CTA owns 32 columns; its 8 warps take every 8th
 // partial (independent, coalesced 128-byte loads) and meet in shared memory: a chain of nparts / 8 loads per thread
-// instead of nparts (the one-thread-per-column version took 31 us for 296 partials, ncu r02).
+// instead of nparts.
 __global__ void __launch_bounds__(256)
 ln_param_reduce_kernel(const float* __restrict__ part, int nparts, int D, int nacc, float* __restrict__ dgamma,
                        float* __restrict__ dbeta, float* __restrict__ dxsum) {
@@ -317,7 +317,7 @@ __global__ void round_tf32_kernel(const float* __restrict__ in, float* __restric
   }
 }
 
-// lo = x - trunc_tf32(x): the part of an fp32 operand the tensor core drops (kind::tf32 truncates to 10 mantissa
+// lo = x - trunc_tf32(x): the part of an fp32 operand the tensor core drops (a tf32 MMA truncates to 10 mantissa
 // bits); exact in fp32.  The 3xTF32 product adds A_lo.B + A.B_lo to A.B.
 __global__ void split_tf32_lo_kernel(const float* __restrict__ in, float* __restrict__ lo, long long n4) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
@@ -571,7 +571,7 @@ int to_half(const float* in, void* out, long long n, const float* scale_ptr, cud
   return 0;
 }
 
-constexpr int kAbsmaxBlocks = 1184;   // 148 SMs x 8
+constexpr int kAbsmaxBlocks = 1056;   // 132 SMs x 8
 size_t grad_scale_workspace_bytes() { return kAbsmaxBlocks * sizeof(unsigned); }
 int grad_scale(const float* g, long long n, int target_log2, float* scale2, void* workspace, size_t ws_bytes, cudaStream_t stream) {
   B200_CHECK_ARG(n > 0 && n % 4 == 0, "grad_scale: n %% 4");

@@ -1,6 +1,6 @@
 // Stage-2 (class-conditional GPT over the code grid: reference enhancing/modules/stage2/layers.py) -- the pieces its
-// blocks need beyond the stage-1 kernels.  The seven Linear layers of a block run on the tcgen05 GEMMs of gemm_tc.cu, the
-// masked attention core on attention_tc.cu / attention_exact.cu (attention_causal_*), LayerNorm on rowwise.cu.  Here:
+// blocks need beyond the stage-1 kernels.  The seven Linear layers of a block run on the tensor-core GEMMs of gemm_tc.cu, the
+// masked attention core on attention_exact.cu (attention_causal_*), LayerNorm on rowwise.cu.  Here:
 //   time_mix     x * w + shift(x) * (1 - w), shift = one step along T with a zero first row   (layers.py:50-58)
 //   sqrelu       square(relu(x)) and its derivative                                           (layers.py:108)
 //   token_embed  cat(tok_emb_cond(conds) + pos_emb_cond, tok_emb_code(codes) + pos_emb_code)  (layers.py:199-206)

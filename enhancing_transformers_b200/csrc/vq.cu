@@ -60,14 +60,11 @@ __device__ __forceinline__ float4 normalize8(const float4& v, float& nrm, int us
   nrm = fmaxf(sqrtf(group8_sum(dot4(v, v))), kNormEps);
   return make_float4(v.x / nrm, v.y / nrm, v.z / nrm, v.w / nrm);
 }
-// two independent fp32 FMAs in one instruction (FFMA2, sm_100): d.x += a * b.x, d.y += a * b.y -- each lane rounds
-// exactly like a scalar fmaf, so the distances (and therefore the argmin) are bit-identical to the scalar loop,
-// at half the FMA issue slots.
+// two independent fp32 FMAs: d.x += a * b.x, d.y += a * b.y, each rounded like a scalar fmaf, so the distances (and
+// therefore the argmin) are bit-identical to the scalar loop
 __device__ __forceinline__ void ffma2(float2& d, float a, const float2 b) {
-  const float2 aa = make_float2(a, a);
-  asm("fma.rn.f32x2 %0, %1, %2, %0;"
-      : "+l"(reinterpret_cast<unsigned long long&>(d))
-      : "l"(reinterpret_cast<const unsigned long long&>(aa)), "l"(reinterpret_cast<const unsigned long long&>(b)));
+  d.x = fmaf(a, b.x, d.x);
+  d.y = fmaf(a, b.y, d.y);
 }
 
 __device__ __forceinline__ void cp_async16(void* dst, const void* src, bool valid) {

@@ -6,16 +6,16 @@ config 2'): LayerNorm statistics, one copy of qkv, the attention output and its 
 Precision modes (`set_precision`, env B200VQ_PRECISION):
 
   "fp16"    default.  The four projections of every transformer block and their dgrad / wgrad run as
-            tcgen05 kind::f16 GEMMs: operands are stored in fp16 by the kernel that produces them
+            f16 tensor-core GEMMs: operands are stored in fp16 by the kernel that produces them
             (LayerNorm, tanh epilogue, attention epilogue), accumulation / residual stream / LayerNorm /
             softmax / losses stay fp32.  fp16 has the same 11-bit significand as tf32, so the results
             carry tf32-level rounding at twice the tensor-core rate and half the operand traffic.
             Gradient operands are multiplied by a power of two S chosen on the device from the gradient
             entering each transformer stack (`ops.grad_scale`) and every fp32 result is multiplied by 1/S
             in the producing epilogue: exact, and it keeps fp16's exponent range out of the picture.
-            The attention core runs on kind::f16 as well (dim_head 64: attention_f16.cu; other head sizes on the kind::tf32
+            The attention core takes fp16 operands as well (dim_head 64: the fp16 core; other head sizes on the tf32
             kernels from a tf32-rounded fp32 qkv matrix).
-  "tf32"    every GEMM on kind::tf32 with operands rounded to nearest where they are produced
+  "tf32"    every GEMM on tf32 tensor cores with operands rounded to nearest where they are produced
             (round 1's data path).
   "parity"  error-compensated 3xTF32 GEMMs and attention (fp32-grade, ~3-6x slower): the mode the
             reference-parity tests use to show margin against the 1e-3 tolerance.
@@ -183,7 +183,7 @@ LAYER_PARAMS = 11
 # always run as 3xTF32: their rounding is not averaged out by anything downstream (to_pixel writes the pixels the
 # 1e-3 tolerance is measured on), and the extra passes cost ~1 ms per 250 ms step.
 PRECISE_IO = os.environ.get("B200VQ_PRECISE_IO", "1") != "0"
-ATTENTION_F16 = os.environ.get("B200VQ_ATTENTION_F16", "1") != "0"   # fp16 mode: kind::f16 attention core for dim_head 64
+ATTENTION_F16 = os.environ.get("B200VQ_ATTENTION_F16", "1") != "0"   # fp16 mode: fp16-operand attention core for dim_head 64
 
 
 def f16_supported(dim: int, inner: int, mlp: int) -> bool:
@@ -261,10 +261,10 @@ def _block_fwd_f16(x, prm, dims):
     wq, wo, w1h, w2h = (weight_shadow(w, "f16") for w in (w_qkv, w_out, w1, w2))
     h1, mean1, rstd1 = ops.layernorm_fwd(x, ln1_w, ln1_b, False, out_half=True)
     if dh == 64 and ATTENTION_F16:
-        qkv = ops.gemm(h1, wq, M, 3 * inner, D, out_half=True, cta_group=cg)              # fp16 qkv -> kind::f16 attention core
+        qkv = ops.gemm(h1, wq, M, 3 * inner, D, out_half=True, cta_group=cg)              # fp16 qkv -> fp16 attention core
         o, lse = ops.attention_f16_fwd(qkv, B, N, heads, dh, scale)
     else:
-        qkv = ops.gemm(h1, wq, M, 3 * inner, D, round_out=True, cta_group=cg)             # fp32, tf32-rounded: kind::tf32 attention core
+        qkv = ops.gemm(h1, wq, M, 3 * inner, D, round_out=True, cta_group=cg)             # fp32, tf32-rounded: tf32 attention core
         o, lse = ops.attention_fwd(qkv, B, N, heads, dh, scale, False, out_half=True)
     x1 = ops.gemm(o, wo, M, D, inner, bias=b_out, res=x, cta_group=cg)
     h2, mean2, rstd2 = ops.layernorm_fwd(x1, ln2_w, ln2_b, False, out_half=True)

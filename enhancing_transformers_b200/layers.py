@@ -153,7 +153,7 @@ class Transformer(nn.Module):
 
 class QuantLinear(nn.Linear):
     """``pre_quant`` / ``post_quant`` of the unchanged ``ViTVQ`` (reference vitvqgan.py:38-39,63,69) on the
-    tcgen05 GEMM instead of cuBLAS.  Same parameters and state-dict keys as the ``nn.Linear`` it replaces
+    tensor-core GEMM (gemm_tc.cu) instead of cuBLAS.  Same parameters and state-dict keys as the ``nn.Linear`` it replaces
     (`from_linear` shares them).  Always the error-compensated 3xTF32 product: ``pre_quant`` writes the
     vector whose nearest code is looked up, so its rounding decides the indices, and both GEMMs are
     memory-bound (K or N = 32) -- the extra tensor passes are free."""

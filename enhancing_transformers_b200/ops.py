@@ -64,7 +64,7 @@ def gemm(a: Tensor, b: Tensor, M: int, N: int, K: int, *, a_major: int = 0, b_ma
     """C[M,N] = epilogue(alpha * A . B^T).  See include/b200vq.h.  With splits > 1 returns [splits, M, N].
     The operand dtype picks the tensor-core flavour: fp32 -> b200vq_gemm_tf32 (or, with a_lo/b_lo, the
     error-compensated b200vq_gemm_3xtf32), fp16 -> b200vq_gemm_f16 (out_half: fp16 C; alpha: device scalar).
-    want_colsum: also return colsum(C) (-> (C, colsum)); the epilogue emits per-32-row partial sums."""
+    want_colsum: also return colsum(C) (-> (C, colsum)); the epilogue emits per-16-row partial sums."""
     half = a.dtype == _HALF
     _req(a, "a", a.dtype if half else torch.float32); _req(b, "b", a.dtype)
     _req(bias, "bias"); _req(res, "res"); _req(alpha, "alpha")
@@ -77,7 +77,7 @@ def gemm(a: Tensor, b: Tensor, M: int, N: int, K: int, *, a_major: int = 0, b_ma
     if out is None:
         out = torch.empty((splits, M, N) if splits > 1 else (M, N), device=a.device, dtype=_HALF if out_half else torch.float32)
     _req(out, "out", _HALF if out_half else torch.float32)
-    part = torch.empty((M + 31) // 32, N, device=a.device, dtype=torch.float32) if want_colsum else None
+    part = torch.empty((M + 15) // 16, N, device=a.device, dtype=torch.float32) if want_colsum else None
     L = _lib.lib()
     ldres = res.shape[-1] if res is not None else 0
     ldaux = aux.shape[-1] if aux is not None else 0
@@ -118,13 +118,14 @@ def splitk_reduce(part: Tensor, out: Optional[Tensor] = None, alpha: Optional[Te
     return out
 
 
-def pick_splits(k_total: int, out_rows: int, out_cols: int, sms: int = 148, k_atom: int = 32) -> int:
+def pick_splits(k_total: int, out_rows: int, out_cols: int, sms: int = 132, k_atom: int = 32) -> int:
     """split count for a wgrad GEMM, by a two-term cost model.  The persistent kernel runs ceil(tiles * splits / sms) waves
-    of 128 x 256 tiles, so the contraction costs flops / (peak * fill of the last wave) (to_qkv's 54 tiles: 4 splits = 1.46
-    waves, 8 splits = 2.92); the partial sums cost one fp32 write and one read per split.  Each split contracts a multiple
-    of one k-block (32 fp32 / 64 fp16 elements) and at least 256 rows."""
-    tiles = -(-out_rows // 128) * -(-out_cols // 256)
-    peak = 1.3e15 if k_atom == 64 else 0.7e15          # kind::f16 / kind::tf32 issue rates (DESIGN.md section 7)
+    of 128 x 128 tiles (one CTA per SM), so the contraction costs flops / (peak * fill of the last wave) (to_qkv's wgrad,
+    a 2304 x 768 output: 108 tiles, 1 split = 0.82 waves, 2 splits = 1.64, 4 splits = 3.27); the partial sums cost one fp32
+    write and one read per split.  Each split contracts a multiple of one k-block (32 fp32 / 64 fp16 elements) and at least
+    256 rows."""
+    tiles = -(-out_rows // 128) * -(-out_cols // 128)
+    peak = 0.99e15 if k_atom == 64 else 0.495e15       # H100 SXM dense f16 / tf32 tensor rates (data sheet)
     t_mma = 2.0 * k_total * out_rows * out_cols / peak
     best, best_t = 1, float("inf")
     s = 1

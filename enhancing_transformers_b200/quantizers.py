@@ -78,7 +78,7 @@ class GumbelQuantizer(BaseQuantizer):
     """Drop-in for the reference's ``GumbelQuantizer`` (quantizers.py:95-126; used by ``ViTVQGumbel``, vitvqgan.py:147-176).
 
     Same constructor and the same ``(z_q, kl-to-uniform loss, indices)`` triple.  The two contractions -- the
-    [tokens, n_embed] logit matrix ``-|z|^2 - |e|^2 + 2 z e^T`` and ``soft_one_hot @ codebook`` -- run on the tcgen05 GEMM
+    [tokens, n_embed] logit matrix ``-|z|^2 - |e|^2 + 2 z e^T`` and ``soft_one_hot @ codebook`` -- run on the tensor-core GEMM
     (3xTF32: the logits feed a softmax with temperature, so they keep fp32-grade accuracy); the Gumbel noise, the softmax
     and the KL term are PyTorch (``F.gumbel_softmax`` draws from the same generator as the reference, so a seeded run
     reproduces the reference's samples up to the rounding of the logits).  Unlike the arg-min lookup this quantiser is

@@ -5,13 +5,13 @@ Same constructor keywords (``stage2/transformer.py:41`` instantiates the YAML's 
 ``forward(codes, conds) -> logits`` / ``sample`` / ``sample_step`` signatures, same ``state_dict`` keys and
 shapes, same module classes (``configure_optimizers`` sorts parameters by ``isinstance(m, nn.Linear)`` etc.,
 ``stage2/transformer.py:141-160``), but every FLOP runs in libb200vq.so: the seven Linear layers of a block and
-the vocabulary head on the tcgen05 GEMMs, the masked attention core on the tcgen05 / 3xTF32 kernels with the
+the vocabulary head on the tensor-core GEMMs, the masked attention core on the tf32 / 3xTF32 kernels with the
 causal + visible-prefix mask folded in, time-shift mixing, squared ReLU, embeddings and the logits window as
 HBM streams (csrc/stage2.cu).
 
-Data path (``etb.set_precision``): "fp16" (default) -> the Linear layers on kind::f16 GEMMs (fp16 operands, fp32 accumulate and
-output, per-call power-of-two gradient scaling chosen on the device), attention core on kind::tf32; "tf32" -> everything
-kind::tf32; "parity" -> 3xTF32 GEMMs and attention (fp32-grade).  Limits of the kernels underneath, raised at construction:
+Data path (``etb.set_precision``): "fp16" (default) -> the Linear layers on f16 GEMMs (fp16 operands, fp32 accumulate and
+output, per-call power-of-two gradient scaling chosen on the device), attention core on tf32; "tf32" -> everything
+tf32; "parity" -> 3xTF32 GEMMs and attention (fp32-grade).  Limits of the kernels underneath, raised at construction:
 head size ``embed_dim // n_heads`` must be 32 or 64, ``embed_dim`` <= 2048, ``vocab_img_size`` % 64 == 0 (the YAML's 6144 / 16 = 384-wide heads --
 a 10.9 B-parameter model that cannot train under replicated fp32 DDP anyway, SURVEY.md section 8f-3 -- are not covered).
 
@@ -132,7 +132,7 @@ class LinearResFn(torch.autograd.Function):
 
 
 class LinearF16Fn(torch.autograd.Function):
-    """x W^T + b (+ res) with fp16 tensor-core operands and fp32 accumulation / output (kind::f16: tf32's 11-bit significand
+    """x W^T + b (+ res) with fp16 tensor-core operands and fp32 accumulation / output (fp16: tf32's 11-bit significand
     at twice the tensor rate and half the operand bytes -- DESIGN.md section 2).  Self-contained gradient scaling: backward
     picks the power of two S that puts max|g| at 2^6 on the device (`ops.grad_scale`, no host sync), feeds fp16(g S) to the
     dgrad / wgrad GEMMs and multiplies their fp32 results by 1/S in the epilogue (exact)."""

@@ -1,4 +1,4 @@
-/* b200vq.h -- C ABI of libb200vq.so: the B200 (sm_100a) kernels behind the ViT-VQGAN hot path of
+/* b200vq.h -- C ABI of libb200vq.so: the H100 (sm_90a) kernels behind the ViT-VQGAN hot path of
  * thuanz123/enhancing-transformers.
  *
  * Boundary (SURVEY.md section 8b).  The reference has no FFI of its own on this path: its
@@ -16,7 +16,7 @@
  *     available from b200vq_last_error() (thread local);
  *   - matrices are row-major with an explicit leading dimension in elements;
  *   - `round_out != 0` stores values rounded to tf32 (round-to-nearest, fp32 container) because
- *     the tensor is only ever consumed as a tcgen05 kind::tf32 operand, which would otherwise
+ *     the tensor is only ever consumed as a tf32 tensor-core operand, which would otherwise
  *     truncate the low 13 mantissa bits;
  *   - fp16 buffers (void*) are plain IEEE binary16 arrays; they only ever hold GEMM operands.
  */
@@ -34,7 +34,7 @@ extern "C" {
 
 int b200vq_version(void);
 const char* b200vq_last_error(void);
-/* compiled-for architecture string, e.g. "sm_100a" */
+/* compiled-for architecture string, e.g. "sm_90a" */
 const char* b200vq_arch(void);
 /* number of kernel launches issued through this library since load (bench.py's gpu_launches) */
 long long b200vq_launch_count(void);
@@ -43,7 +43,7 @@ long long b200vq_launch_count(void);
  * variable B200VQ_SM_LIMIT. */
 int b200vq_set_sm_limit(int n);
 
-/* ---- GEMM: C[M,N] = epi( alpha * A . B^T ) on tcgen05 tensor cores, fp32 accumulate ------------------
+/* ---- GEMM: C[M,N] = epi( alpha * A . B^T ) on mma.sync tensor cores, fp32 accumulate ------------------
  * Replaces nn.Linear / Conv2d(k=s) / ConvTranspose2d(k=s) forward, dgrad and wgrad:
  *   layers.py:99-101 (FeedForward), :118,:120 (to_qkv, to_out), :169 (patch embed), :204 (to_pixel),
  *   vitvqgan.py:38-39 (pre_quant / post_quant).
@@ -53,16 +53,16 @@ int b200vq_set_sm_limit(int n);
  * Epilogue, in this order: * alpha; + bias[N]; act (0 none, 1 tanh -- layers.py:100);
  * * (1 - aux^2) (tanh backward); + res[row % res_row_mod or row] (residual add layers.py:147-148
  * or positional table :179,:210); tf32 rounding / fp16 conversion.
- * colsum_part (nullable, [ceil(M/32)][N], splits must be 1): receives the column sums of every 32-row group of
+ * colsum_part (nullable, [ceil(M/16)][N], splits must be 1): receives the column sums of every 16-row group of
  * the stored C -- summed over the groups (b200vq_colsum) they are the bias gradient of the Linear whose
  * pre-activation gradient this GEMM produced (net.0, layers.py:99), without another pass over C.
  * cta_group: 1 = one CTA per 128 x bn tile, 2 = CTA pair per 256 x bn tile; bn in {0=auto,64,128,192,256}.
  *
  * Three operand flavours:
- *   gemm_tf32   A, B fp32, kind::tf32 (10-bit mantissa; the hardware truncates, so producers round to nearest).
+ *   gemm_tf32   A, B fp32, tf32 MMA (10-bit mantissa; the hardware truncates, so producers round to nearest).
  *   gemm_3xtf32 A, B fp32 plus their truncation residues A_lo, B_lo (b200vq_split_tf32_lo): the
  *               error-compensated product A_lo.B + A.B_lo + A.B -- fp32-grade, used by precision="parity".
- *   gemm_f16    A, B fp16 (kind::f16: the same 11-bit significand as tf32 at twice the tensor rate and half the
+ *   gemm_f16    A, B fp16 (f16 MMA: the same 11-bit significand as tf32 at twice the tensor rate and half the
  *               operand bytes); C fp32, or fp16 when out_half (then aux is fp16 too; no residual / split-K).
  *               alpha (device scalar, nullable) undoes the power-of-two scale fp16 gradient operands carry. */
 int b200vq_gemm_tf32(const float* A, long long lda, int a_major, const float* B, long long ldb, int b_major,
@@ -111,7 +111,7 @@ int b200vq_attention_bwd(const float* qkv, const void* out, int out_half, const 
                          void* dqkv, int dqkv_half, const float* dqkv_scale, float* delta, int B, int N, int heads,
                          int dh, float scale, int round_out, void* stream);
 /* fp16-operand core (dh == 64): qkv16 / out16 / dout16 / dqkv16 are fp16 matrices of the shapes above; tensor-core
- * operands fp16 (kind::f16), scores / softmax / accumulation fp32.  dout16 carries the power-of-two gradient scale of
+ * operands fp16, scores / softmax / accumulation fp32.  dout16 carries the power-of-two gradient scale of
  * the backward segment and dqkv16 comes out with the same scale (everything is linear in dout). */
 int b200vq_attention_f16_fwd(const void* qkv16, void* out16, float* lse, int B, int N, int heads, int dh, float scale,
                              void* stream);
@@ -157,7 +157,7 @@ int b200vq_add_rows_mod(const float* x, const float* table, float* out, long lon
 
 
 /* ---- operand preparation for the 3xTF32 and fp16 data paths --------------------------------------*/
-/* lo = in - trunc_tf32(in): the bits kind::tf32 drops (exact in fp32) */
+/* lo = in - trunc_tf32(in): the bits a tf32 MMA drops (exact in fp32) */
 int b200vq_split_tf32_lo(const float* in, float* lo, long long n, void* stream);
 /* out16 = fp16(in * *scale), saturating at +-65504 (scale: device scalar or NULL) */
 int b200vq_to_half(const float* in, void* out16, long long n, const float* scale, void* stream);
@@ -184,7 +184,7 @@ int b200vq_upfirdn2d(const float* in, const float* kernel, float* out, long long
  * attention_causal: the stage-1 attention contract (same packed qkv / out / lse / delta layouts, fp32) with the stage-2
  *   mask of layers.py:43-48,83-85: query q attends to key k iff k <= max(q, cond_len - 1) -- causal, the cond_len
  *   condition tokens fully visible to each other.  exact != 0: error-compensated 3xTF32 (precision="parity");
- *   otherwise the tcgen05 kind::tf32 kernels (round_out as in b200vq_attention_fwd).  dh (the head size
+ *   otherwise the single-pass tf32 kernels (round_out as in b200vq_attention_fwd).  dh (the head size
  *   embed_dim / n_heads) must be 32 or 64.
  * time_mix: y = x * w + shift(x) * (1 - w), shift = one step along T with a zero first row (layers.py:50-58), bit-identical
  *   to the reference's four fp32 tensor ops.  x, y [M = B*T, C]; w [C].

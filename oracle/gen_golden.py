@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz by running the UNMODIFIED reference modules.
 
-Runs only in the build container (needs /root/reference).  The reference is imported by file
+Needs a checkout of the reference (B200VQ_REFERENCE).  The reference is imported by file
 path (its package __init__ pulls in pytorch_lightning / omegaconf, absent here -- SURVEY.md
 section 8c) with one harness-side shim: ``np.float = float`` (reference layers.py:57 uses the
 alias numpy removed in 1.24).  No reference source is copied; only its outputs are stored.
@@ -18,7 +18,10 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-REF = os.environ.get("B200VQ_REFERENCE", "/root/reference")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import vitvq_oracle as O  # noqa: E402
+
+REF = os.environ.get("B200VQ_REFERENCE", "")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 
@@ -84,7 +87,7 @@ def gen_vit(L, Q):
     with torch.no_grad():
         q = vq.norm(vq.embedding(idx))
         out["decode_codes"] = dec(post(q)).numpy()
-    np.savez_compressed(os.path.join(OUT, "vit_tiny.npz"), **out)
+    O.save_golden(os.path.join(OUT, "vit_tiny.npz"), out)       # more than 1 MB: vit_tiny.npz + continuation files
     print("vit_tiny: loss", float(loss), "qloss", float(qloss), "distinct codes", idx.unique().numel())
 
 
@@ -210,7 +213,7 @@ def gen_lossops():
 
 if __name__ == "__main__":
     if not os.path.isdir(REF):
-        sys.exit(f"{REF} not present: golden vectors can only be generated in the build container")
+        sys.exit(f"{REF} not present: golden vectors need a reference checkout (B200VQ_REFERENCE)")
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(4)
     L, Q = load_reference()

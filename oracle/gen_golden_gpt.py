@@ -1,5 +1,5 @@
 """Generate tests/golden/gpt_tiny.npz by running the UNMODIFIED reference stage-2 ``GPT``
-(/root/reference/enhancing/modules/stage2/layers.py).  Runs only in the build container.
+(enhancing/modules/stage2/layers.py of a reference checkout, B200VQ_REFERENCE).
 
 The file is imported by path (the package __init__ needs pytorch_lightning); its one absent import, ``omegaconf`` (used
 for a type annotation only), is stubbed in sys.modules.  No reference source is copied; only outputs are stored.
@@ -16,7 +16,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-REF = os.environ.get("B200VQ_REFERENCE", "/root/reference")
+REF = os.environ.get("B200VQ_REFERENCE", "")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 CFG = dict(vocab_cond_size=10, vocab_img_size=64, embed_dim=64, cond_num_tokens=2, img_num_tokens=30, n_heads=2, n_layers=2)
@@ -81,6 +81,6 @@ def main():
 
 if __name__ == "__main__":
     if not os.path.isdir(REF):
-        sys.exit(f"{REF} not present: golden vectors can only be generated in the build container")
+        sys.exit(f"{REF} not present: golden vectors need a reference checkout (B200VQ_REFERENCE)")
     torch.set_num_threads(4)
     main()

@@ -6,12 +6,12 @@ reference's ``enhancing/modules/stage1/layers.py`` (ViTEncoder / ViTDecoder) and
 ``nn.Linear`` layers the reference's ``ViTVQ`` LightningModule puts between them
 (``vitvqgan.py:38-39,63,69``).  It exists so that ``tests/``, ``__graft_entry__.smoke()`` and
 ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs have something to check the CUDA path
-against on a machine where ``/root/reference`` does not exist.  Nothing under the product
+against on a machine without a reference checkout.  Nothing under the product
 package (``enhancing_transformers_b200/``) may import it.
 
 Parity pin: the reference ships no tests and no golden vectors (SURVEY.md section 4), so this
-oracle is pinned against outputs of the *reference itself*, generated in the build container by
-``oracle/gen_golden.py`` (which imports the reference modules from ``/root/reference`` by file
+oracle is pinned against outputs of the *reference itself*, generated from a reference checkout by
+``oracle/gen_golden.py`` (which imports the reference modules from a reference checkout by file
 path) and committed under ``tests/golden/``.  ``tests/test_oracle_golden.py`` replays them.
 
 Arithmetic: fp32 torch CPU ops (the reference's own arithmetic lives in ATen, SURVEY.md
@@ -396,3 +396,59 @@ def flops_per_image(cfg: dict) -> float:
                + 2 * e["dim"] * q["embed_dim"] + 2 * q["embed_dim"] * d["dim"]
                + T * 2 * q["embed_dim"] * q["n_embed"])
     return float(n * per_tok)
+
+
+# the config of tests/golden/ref_vitvq_small.npz: residual VQ, unequal encoder / decoder depths, dim_head != dim / heads
+SMALL_REF_CFG = dict(image_size=48, patch_size=8, encoder=dict(dim=64, depth=2, heads=2, mlp_dim=96, dim_head=32),
+                     decoder=dict(dim=64, depth=1, heads=2, mlp_dim=64, dim_head=32),
+                     quantizer=dict(embed_dim=32, n_embed=128, use_residual=True, num_quantizers=2))
+
+
+def seeded_gumbel_softmax(seed: int):
+    """a drop-in for F.gumbel_softmax (same formula as torch's) whose noise comes from a CPU generator seeded with `seed`:
+    a run on any device draws the same noise, so a GPU module can be compared with a golden recorded on the CPU"""
+    gen = torch.Generator().manual_seed(seed)
+
+    def gumbel_softmax(logits, tau=1.0, hard=False, eps=1e-10, dim=-1):
+        g = -torch.empty(logits.shape, dtype=torch.float32).exponential_(generator=gen).log()
+        y = ((logits + g.to(device=logits.device, dtype=logits.dtype)) / tau).softmax(dim)
+        if hard:
+            index = y.max(dim, keepdim=True)[1]
+            return torch.zeros_like(logits).scatter_(dim, index, 1.0) - y.detach() + y
+        return y
+    return gumbel_softmax
+
+
+class _Golden(dict):
+    @property
+    def files(self):
+        return list(self)
+
+
+def load_golden(path: str) -> "_Golden":
+    """np.load of `path` (an .npz) merged with its continuation files <stem>.1.npz, <stem>.2.npz, ...: a fixture larger
+    than 1 MB is stored in several files.  Offers NpzFile's `.files` / `[key]` interface."""
+    import os
+    out = _Golden(np.load(path))
+    stem = path[:-len(".npz")]
+    i = 1
+    while os.path.exists(f"{stem}.{i}.npz"):
+        out.update(np.load(f"{stem}.{i}.npz"))
+        i += 1
+    return out
+
+
+def save_golden(path: str, arrays: Dict[str, np.ndarray], limit: int = 900_000) -> None:
+    """np.savez_compressed of `arrays` into `path` and as many continuation files as keep each under `limit` bytes of
+    array data (the inverse of load_golden)"""
+    parts, cur, size = [], {}, 0
+    for k, v in arrays.items():
+        if cur and size + v.nbytes > limit:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = v
+        size += v.nbytes
+    parts.append(cur)
+    stem = path[:-len(".npz")]
+    for i, part in enumerate(parts):
+        np.savez_compressed(path if i == 0 else f"{stem}.{i}.npz", **part)

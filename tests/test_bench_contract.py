@@ -1,5 +1,5 @@
 """bench.py contract: the reference arm runs on CPU and prints one JSON line with the required
-keys; the B200 arm (gpu) prints the full line including roofline / e2e / clocks / gpu_launches."""
+keys; the CUDA arm (gpu) prints the full line including roofline / e2e / clocks / gpu_launches."""
 import json
 import os
 import subprocess

@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual C-ABI kernels (run on the B200 box: pytest -m gpu).
+"""GPU parity tests of the individual C-ABI kernels (run on an H100: pytest -m gpu).
 References: exact integer/index parity against the oracle and the golden fixtures; floating
 point against fp64 torch on the same (tf32-pre-rounded, where the tensor cores consume them)
 inputs with the tolerance written at each assert."""
@@ -60,7 +60,7 @@ def test_gemm_epilogues(cg):
 @pytest.mark.parametrize("cg", [1, 2])
 @pytest.mark.parametrize("M,N,K", [(512, 768, 256), (1000, 320, 96), (40, 64, 64), (4096, 3072, 128)])
 def test_gemm_epilogue_column_sums(cg, M, N, K):
-    """the epilogue's per-32-row partial column sums reduce to colsum of the *stored* C (ragged M and N included)"""
+    """the epilogue's per-16-row partial column sums reduce to colsum of the *stored* C (ragged M and N included)"""
     a, bs = tf32_rn(torch.randn(M, K, device="cuda")), tf32_rn(torch.randn(K, N, device="cuda"))
     aux, bias = torch.tanh(torch.randn(M, N, device="cuda")), torch.randn(N, device="cuda")
     c, cs = ops.gemm(a, bs, M, N, K, b_major=1, aux=aux, bias=bias, round_out=True, cta_group=cg, want_colsum=True)
@@ -103,7 +103,7 @@ def test_gemm_tn_wgrad_form_with_split_k(cg, M, N, K, splits):
 
 
 def test_gemm_hardware_truncates_unrounded_operands():
-    """documents why operands are pre-rounded: tcgen05 kind::tf32 drops the low 13 mantissa bits"""
+    """documents why operands are pre-rounded: a tf32 MMA drops the low 13 mantissa bits"""
     a, b = torch.randn(256, 256, device="cuda"), torch.randn(256, 256, device="cuda")
     c = ops.gemm(a, b, 256, 256, 256)
     trunc = lambda t: (t.view(torch.int32) & ~0x1fff).view(torch.float32)

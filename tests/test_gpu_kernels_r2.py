@@ -1,5 +1,5 @@
 """GPU parity tests of the round-2 kernels (pytest -m gpu, through the C ABI): the fp16-operand GEMM
-(kind::f16) and its fp16 epilogue, the error-compensated 3xTF32 GEMM, the 3xTF32 attention core, the fp16
+(f16 tensor cores) and its fp16 epilogue, the error-compensated 3xTF32 GEMM, the 3xTF32 attention core, the fp16
 outputs of LayerNorm / attention, the device-side gradient scale, the un-normalised quantiser and the
 contention-proof codebook scatter.  Floating-point references are fp64 torch on identical (pre-rounded)
 inputs; the tolerance is written at each assert."""
@@ -283,7 +283,7 @@ def test_attention_f16_fwd_bwd(B, N, heads):
 
 
 def test_attention_f16_matches_tf32_core():
-    """same inputs through the kind::tf32 core (fp16 values are exactly representable in tf32): outputs agree to
+    """same inputs through the tf32 core (fp16 values are exactly representable in tf32): outputs agree to
     fp16 rounding, i.e. the fp16 core loses nothing against the tf32 one"""
     B, N, heads, dh = 2, 512, 3, 64
     inner = heads * dh

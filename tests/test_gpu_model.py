@@ -84,9 +84,9 @@ GRAD_TOL = {"fp16": 5e-3, "tf32": 5e-3, "parity": 1e-4}
 
 @pytest.mark.parametrize("mode", MODES)
 def test_against_reference_golden_fwd_bwd(golden_dir, mode):
-    """the reference's own outputs (tests/golden/vit_tiny.npz, written by oracle/gen_golden.py from /root/reference)"""
+    """the reference's own outputs (tests/golden/vit_tiny.npz, written by oracle/gen_golden.py from the reference checkout)"""
     etb.set_precision(mode)
-    g = np.load(os.path.join(golden_dir, "vit_tiny.npz"))
+    g = O.load_golden(os.path.join(golden_dir, "vit_tiny.npz"))
     sd = {k[3:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd.")}
     mods = build(GOLD_CFG, sd)
     loss, rec, idx, h, z = run(mods, torch.from_numpy(g["img"]).cuda())
@@ -125,7 +125,7 @@ def test_post_quant_with_positional_table_in_the_epilogue(golden_dir, mode):
     the decoder skips its own add.  Same fp32 operations in the same order as the separate path: identical reconstruction,
     identical decode_codes (vs the reference golden too), identical gradients; state-dict keys unchanged."""
     etb.set_precision(mode)
-    g = np.load(os.path.join(golden_dir, "vit_tiny.npz"))
+    g = O.load_golden(os.path.join(golden_dir, "vit_tiny.npz"))
     sd = {k[3:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd.")}
     img = torch.from_numpy(g["img"]).cuda()
     gidx = torch.from_numpy(g["idx"]).cuda()
@@ -475,82 +475,62 @@ def test_frozen_model_backward_skips_parameter_gradients():
     assert n_frozen < etb.ops.launch_count() - n0
 
 
-def test_non_square_patches_match_the_reference_modules():
-    """reference layers.py:157-166 accepts (height, width) patches; checked against the vendored reference modules
-    (oracle/_ref, built by oracle/build_ref.py) on the CPU"""
-    import importlib.util
-    ref_dir = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "enhancing_ref")
-    if not os.path.exists(os.path.join(ref_dir, "layers.py")):
-        pytest.skip("oracle/_ref not present")
-    if not hasattr(np, "float"):
-        np.float = float
-    spec = importlib.util.spec_from_file_location("enhancing_ref_ns.layers", os.path.join(ref_dir, "layers.py"))
-    RL = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(RL)
+def test_non_square_patches_match_the_reference_modules(golden_dir):
+    """reference layers.py:157-166 accepts (height, width) patches; checked against the reference modules' own outputs
+    (tests/golden/ref_nonsquare.npz, written on the CPU by oracle/gen_golden_ref_modules.py)"""
+    g = np.load(os.path.join(golden_dir, "ref_nonsquare.npz"))
     etb.set_precision("parity")
-    torch.manual_seed(0)
     kw = dict(image_size=(32, 48), patch_size=(8, 4), dim=64, depth=1, heads=2, mlp_dim=128, dim_head=32)
-    ref_e, ref_d = RL.ViTEncoder(**kw), RL.ViTDecoder(**kw)
     enc, dec = etb.ViTEncoder(**kw), etb.ViTDecoder(**kw)
-    enc.load_state_dict(ref_e.state_dict(), strict=True); dec.load_state_dict(ref_d.state_dict(), strict=True)
+    enc.load_state_dict({k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("enc.")}, strict=True)
+    dec.load_state_dict({k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("dec.")}, strict=True)
     enc.cuda(); dec.cuda()
-    img = torch.rand(2, 3, 32, 48)
-    h_ref = ref_e(img)
-    rec_ref = ref_d(h_ref)
-    h = enc(img.cuda())
+    h_ref, rec_ref = torch.from_numpy(g["h"]), torch.from_numpy(g["rec"])
+    h = enc(torch.from_numpy(g["img"]).cuda())
     assert h.shape == h_ref.shape == (2, 48, 64)
-    assert relmax(h.cpu(), h_ref.detach()) < 5e-5
-    assert relmax(dec(h).cpu(), rec_ref.detach()) < 5e-5
+    assert relmax(h.cpu(), h_ref) < 5e-5
+    assert relmax(dec(h).cpu(), rec_ref) < 5e-5
     with pytest.raises(NotImplementedError, match="multiple of 4"):
         etb.ViTEncoder(image_size=30, patch_size=6, dim=64, depth=1, heads=2, mlp_dim=64)
 
 
 @pytest.mark.parametrize("residual", [False, True])
-def test_gumbel_quantizer_matches_reference(residual):
-    """reference quantizers.py:95-126 (SURVEY.md section 8 f-4).  The quantiser is stochastic; with the generator seeded
-    identically F.gumbel_softmax draws the same noise on the same device, so the soft sample, the KL loss and the
-    gradients of the vendored reference class (oracle/_ref, moved to the GPU, TF32 matmuls off) are reproduced up to
-    the rounding of the logits; in eval mode (hard one-hot of a noisy arg-max) the indices agree except at near-ties."""
-    import importlib.util
-    ref_dir = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "enhancing_ref")
-    if not os.path.exists(os.path.join(ref_dir, "quantizers.py")):
-        pytest.skip("oracle/_ref not present")
-    spec = importlib.util.spec_from_file_location("enhancing_ref_ns.quantizers", os.path.join(ref_dir, "quantizers.py"))
-    RQ = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(RQ)
+def test_gumbel_quantizer_matches_reference(golden_dir, monkeypatch, residual):
+    """reference quantizers.py:95-126 (SURVEY.md section 8 f-4).  The quantiser is stochastic; with the Gumbel noise
+    replayed from the seeded CPU generator the golden was recorded with (tests/golden/ref_gumbel.npz, the reference
+    class on the CPU in fp32), the soft sample, the KL loss and the gradients are reproduced up to the rounding of the
+    logits; in eval mode (hard one-hot of a noisy arg-max) the indices agree except at near-ties."""
+    g = np.load(os.path.join(golden_dir, "ref_gumbel.npz"))
+    tag = "res" if residual else "plain"
+    G = lambda k: torch.from_numpy(g[f"{tag}.{k}"]).cuda()
     torch.backends.cuda.matmul.allow_tf32 = False
     kw = dict(embed_dim=32, n_embed=512, temp_init=0.7, use_residual=residual, num_quantizers=3 if residual else None)
-    torch.manual_seed(0)
-    ref = RQ.GumbelQuantizer(**kw).cuda()
-    ours = etb.GumbelQuantizer(**kw).cuda()
-    ours.load_state_dict(ref.state_dict(), strict=True)
-    z0 = torch.randn(2, 96, 32, device="cuda")
+    ours = etb.GumbelQuantizer(**kw)
+    ours.load_state_dict({k[len(tag) + 4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith(f"{tag}.sd.")}, strict=True)
+    ours.cuda()
+    z0 = G("z0")
     # training mode: soft samples, gradients through the sample
-    outs = []
-    for q in (ref, ours):
-        q.train(); q.zero_grad()
-        z = z0.clone().requires_grad_(True)
-        torch.manual_seed(123)
-        zq, loss, idx = q(z)
-        (zq.square().mean() + loss).backward()
-        outs.append((zq.detach(), loss.detach(), idx, z.grad, q.embedding.weight.grad.clone()))
-    (zq_r, l_r, i_r, gz_r, ge_r), (zq_o, l_o, i_o, gz_o, ge_o) = outs
+    ours.train()
+    z = z0.clone().requires_grad_(True)
+    monkeypatch.setattr(torch.nn.functional, "gumbel_softmax", O.seeded_gumbel_softmax(123))
+    zq_o, l_o, i_o = ours(z)
+    (zq_o.square().mean() + l_o).backward()
+    zq_r, l_r, i_r = G("zq"), G("loss"), G("idx")
     assert zq_o.shape == zq_r.shape and i_o.shape == i_r.shape and i_o.dtype == torch.int64
-    assert relmax(zq_o, zq_r) < 2e-4 and abs(float(l_o - l_r)) < 1e-5 * max(1.0, abs(float(l_r)))
+    assert relmax(zq_o.detach(), zq_r) < 2e-4 and abs(float(l_o - l_r)) < 1e-5 * max(1.0, abs(float(l_r)))
     assert (i_o == i_r).float().mean() > 0.99
-    if gz_r is None:          # residual mode quantises a detached copy of z (quantizers.py:43) and has no straight-through term
-        assert gz_o is None
+    if f"{tag}.gz" not in g.files:   # residual mode quantises a detached copy of z (quantizers.py:43): no straight-through term
+        assert z.grad is None
     else:
-        assert relmax(gz_o, gz_r) < 2e-3
-    assert relmax(ge_o, ge_r) < 2e-3
+        assert relmax(z.grad, G("gz")) < 2e-3
+    assert relmax(ours.embedding.weight.grad, G("gE")) < 2e-3
     # eval mode: hard samples
+    ours.eval()
+    monkeypatch.setattr(torch.nn.functional, "gumbel_softmax", O.seeded_gumbel_softmax(7))
     with torch.no_grad():
-        res = []
-        for q in (ref, ours):
-            q.eval()
-            torch.manual_seed(7)
-            res.append(q(z0))
-    assert (res[0][2] == res[1][2]).float().mean() > 0.99
-    same = (res[0][2] == res[1][2])
+        zq_e, _, idx_e = ours(z0)
+    idx_r = G("eval_idx")
+    assert (idx_e == idx_r).float().mean() > 0.99
+    same = (idx_e == idx_r)
     same = same.all(-1) if residual else same
-    assert relmax(res[1][0][same], res[0][0][same]) < 1e-4
+    assert relmax(zq_e[same], G("eval_zq")[same]) < 1e-4

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import enhancing_transformers_b200 as etb
+from oracle import vitvq_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD_CFG = dict(image_size=32, patch_size=8, encoder=dict(dim=64, depth=2, heads=2, mlp_dim=128),
@@ -41,7 +42,7 @@ def test_vitvq_host_logic_with_emulated_kernels(golden_dir, monkeypatch, mode, f
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import emulated_ops
     emulated_ops.install(monkeypatch)
-    g = np.load(os.path.join(golden_dir, "vit_tiny.npz"))
+    g = O.load_golden(os.path.join(golden_dir, "vit_tiny.npz"))
     sd = {k[3:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd.")}
     prev = etb.set_precision(mode)
     try:

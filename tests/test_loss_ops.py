@@ -1,6 +1,6 @@
 """The loss stage's two native ops (SURVEY.md section 8f-2) against tests/golden/lossops.npz, which oracle/gen_golden.py
 wrote from the REFERENCE's own CPU formulas (losses/op/upfirdn2d.py:168-206, losses/op/fused_act.py:110-122).
-CPU tests pin the module's CPU branch; `-m gpu` tests run the sm_100a kernels through the C ABI (values, first-order
+CPU tests pin the module's CPU branch; `-m gpu` tests run the sm_90a kernels through the C ABI (values, first-order
 gradients and the double-backward an R1-style penalty needs)."""
 import os
 

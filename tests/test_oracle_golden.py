@@ -1,5 +1,5 @@
 """Pins oracle/vitvq_oracle.py against outputs of the unmodified reference
-(tests/golden/*.npz, written by oracle/gen_golden.py in the build container)."""
+(tests/golden/*.npz, written by oracle/gen_golden.py from a reference checkout)."""
 import os
 
 import numpy as np
@@ -79,7 +79,7 @@ def test_quantizer_matches_reference(golden_dir, tag, kw):
 
 
 def test_vitvq_end_to_end_matches_reference(golden_dir):
-    g = _load(golden_dir, "vit_tiny.npz")
+    g = O.load_golden(os.path.join(golden_dir, "vit_tiny.npz"))
     sd = {k[3:]: _t(g[k]).clone().requires_grad_(True) for k in g.files if k.startswith("sd.")}
     cfg = dict(image_size=int(g["cfg_image"]), patch_size=int(g["cfg_patch"]),
                encoder=dict(dim=64, depth=2, heads=2, mlp_dim=128), decoder=dict(dim=96, depth=2, heads=3, mlp_dim=160),
@@ -107,7 +107,7 @@ def test_vitvq_end_to_end_matches_reference(golden_dir):
 
 
 def test_init_sd_has_reference_keys(golden_dir):
-    g = _load(golden_dir, "vit_tiny.npz")
+    g = O.load_golden(os.path.join(golden_dir, "vit_tiny.npz"))
     cfg = dict(image_size=32, patch_size=8, encoder=dict(dim=64, depth=2, heads=2, mlp_dim=128),
                decoder=dict(dim=96, depth=2, heads=3, mlp_dim=160, dim_head=32), quantizer=dict(embed_dim=32, n_embed=256))
     sd = O.init_vitvq_sd(cfg)
@@ -125,46 +125,22 @@ def test_flops_match_baseline_md():
     assert abs(O.flops_per_image(O.CONFIGS["large"]) / 1e9 - 1410.1) < 0.2
 
 
-def test_oracle_matches_the_vendored_reference_modules():
-    """where oracle/_ref exists (oracle/build_ref.py: the reference's own layers.py / quantizers.py, byte for byte) the
-    oracle port is pinned against the live reference modules, fwd + bwd, on a config no fixture covers"""
-    import importlib.util
-    import pytest
+def test_oracle_matches_the_vendored_reference_modules(golden_dir):
+    """the oracle port against the reference's own layers.py / quantizers.py (tests/golden/ref_vitvq_small.npz, written by
+    oracle/gen_golden_ref_modules.py), fwd + bwd, on a config no other fixture covers"""
     import torch
-    ref_dir = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "enhancing_ref")
-    if not os.path.exists(os.path.join(ref_dir, "layers.py")):
-        pytest.skip("oracle/_ref not built (needs /root/reference: python oracle/build_ref.py)")
-    if not hasattr(np, "float"):
-        np.float = float
-    mods = {}
-    for name in ("layers", "quantizers"):
-        spec = importlib.util.spec_from_file_location(f"enhancing_ref_t.{name}", os.path.join(ref_dir, f"{name}.py"))
-        mods[name] = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mods[name])
-    cfg = dict(image_size=48, patch_size=8, encoder=dict(dim=64, depth=2, heads=2, mlp_dim=96, dim_head=32),
-               decoder=dict(dim=64, depth=1, heads=2, mlp_dim=64, dim_head=32),
-               quantizer=dict(embed_dim=32, n_embed=128, use_residual=True, num_quantizers=2))
+    g = np.load(os.path.join(golden_dir, "ref_vitvq_small.npz"))
+    cfg = O.SMALL_REF_CFG
     sd = O.init_vitvq_sd(cfg, seed=7)
-    e, d, q = cfg["encoder"], cfg["decoder"], cfg["quantizer"]
-    ref = dict(encoder=mods["layers"].ViTEncoder(48, 8, **e), decoder=mods["layers"].ViTDecoder(48, 8, **d),
-               quantizer=mods["quantizers"].VectorQuantizer(**q), pre_quant=torch.nn.Linear(64, 32), post_quant=torch.nn.Linear(32, 64))
-    for name, m in ref.items():
-        m.load_state_dict({k[len(name) + 1:]: v for k, v in sd.items() if k.startswith(name + ".")}, strict=True)
     img = torch.rand(2, 3, 48, 48, generator=torch.Generator().manual_seed(3))
-    quant, qloss, idx = ref["quantizer"](ref["pre_quant"](ref["encoder"](img)))
-    rec = ref["decoder"](ref["post_quant"](quant))
-    loss = ((rec - img) ** 2).mean() + qloss
-    loss.backward()
     sdg = {k: v.clone().requires_grad_(v.is_floating_point() and "pos_embedding" not in k) for k, v in sd.items()}
     loss_o, rec_o, idx_o = O.vitvq_loss(sdg, img, cfg)
     loss_o.backward()
-    assert torch.equal(idx, idx_o)
-    torch.testing.assert_close(rec_o, rec, rtol=1e-5, atol=1e-6)
-    torch.testing.assert_close(loss_o, loss, rtol=1e-6, atol=1e-8)
-    for name, m in ref.items():
-        for pn, p in m.named_parameters():
-            g = sdg[f"{name}.{pn}"].grad
-            if p.grad is None:
-                assert g is None or g.abs().max() == 0
-            else:
-                torch.testing.assert_close(g, p.grad, rtol=1e-4, atol=1e-8)
+    assert torch.equal(torch.from_numpy(g["idx"]), idx_o)
+    torch.testing.assert_close(rec_o, torch.from_numpy(g["rec"]), rtol=1e-5, atol=1e-6)
+    torch.testing.assert_close(loss_o, torch.from_numpy(g["loss"]), rtol=1e-6, atol=1e-8)
+    for k, v in sdg.items():
+        if f"grad.{k}" in g.files:
+            torch.testing.assert_close(v.grad, torch.from_numpy(g[f"grad.{k}"]), rtol=1e-4, atol=1e-8)
+        elif v.requires_grad:
+            assert v.grad is None or v.grad.abs().max() == 0, k

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Stage-2 GPT timing on one B200 (development probe, not the bench): fwd+bwd tokens/s of a reduced-width GPT at config 5's
+"""Stage-2 GPT timing on one GPU (development probe, not the bench): fwd+bwd tokens/s of a reduced-width GPT at config 5's
 sequence geometry (1 class token + 1024 codes, 8192-entry vocabulary), CUDA events, per data path.
 
     python tools/stage2_probe.py [embed_dim] [n_layers] [batch]"""
