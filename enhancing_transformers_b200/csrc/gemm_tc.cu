@@ -11,7 +11,7 @@
 //      nearest where they are produced).  With passes == 3 the contraction runs three times over
 //      (A_lo, B), (A, B_lo), (A, B) -- the error-compensated "3xTF32" product (lo = x - trunc_tf32(x),
 //      written by split_tf32_lo): fp32-grade results for the parity mode, at a third of the rate.
-//   1  fp16 storage, wgmma m64nNk16 .f16 straight from the swizzled tiles (either major: wgmma transposes fp16
+//   1  fp16 storage, wgmma m64n256k16 .f16 straight from the swizzled tiles (either major: wgmma transposes fp16
 //      operands itself), fp32 accumulate: the same 11-bit significand as tf32 at twice
 //      the tensor rate and half the operand bytes; gradients travel scaled by a power of two (alpha
 //      undoes it), so fp16's narrower exponent range is never the limit.
@@ -29,7 +29,7 @@
 // by the consumer warps themselves (scalar loads from the swizzled tiles), behind the same TMA ring and epilogue.
 //
 // Warp roles (288 threads): warps 0..7 consume, warp 8 is the TMA producer.  fp16: warpgroup w (warps 4w..4w+3) owns
-// rows 64w .. 64w+63 of the 128 x BN tile (warp 4w+i: rows 64w+16i .. +15); tf32: warp w owns rows 32*(w%4) .. +31
+// rows 64w .. 64w+63 of the 128 x 256 tile (warp 4w+i: rows 64w+16i .. +15); tf32: warp w owns rows 32*(w%4) .. +31
 // and half of the BN columns.
 #include "common.cuh"
 
@@ -61,6 +61,7 @@ struct GemmParams {
 };
 
 constexpr int kBM = 128;
+constexpr int kBNHalf = 256;      // tile width of the fp16 kind (ops.GEMM_TILE mirrors it for the split-K model)
 constexpr int kConsumerWarps = 8;
 constexpr int kGemmThreads = 32 * (kConsumerWarps + 1);
 
@@ -193,6 +194,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
       for (int j = 0; j < NTW; ++j) part[i][j][0] = part[i][j][1] = part[i][j][2] = part[i][j][3] = 0.f;
 
+    float (&d)[BN / 2] = *reinterpret_cast<float(*)[BN / 2]>(&acc[0][0][0]);   // the wgmma accumulator (fp16 kind)
+    int held = -1;                                                            // fp16: the stage of the MMAs in flight
+    if constexpr (WG) wgmma_fence_regs(d);
     for (int kb = 0; kb < kb_total; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       const uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
@@ -229,28 +233,36 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       } else {
-        // one warpgroup-wide MMA per 16-deep k step: A = this warpgroup's 64 rows, B = the whole BN-column tile.
+        // one warpgroup-wide MMA per 16-deep k step: A = this warpgroup's 64 rows, B = the whole 256-column tile.
+        // (256 rather than 128 columns halves the shared-memory B reads per FLOP and the A loads from L2 per FLOP.)
         // K-major: 8-row groups 1024 B apart (SBO), a k step is 32 B along the row.  MN-major: 64-element atoms
         // kBK*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO), a k step is 16 k-rows = 2048 B.
         const int wg = warp >> 2;
         const uint32_t sa_u = smem_base + stage * Cfg::STAGE_BYTES, sb_u = sa_u + Cfg::A_BYTES;
         const uint32_t a0 = sa_u + wg * (AMAJ ? kBK * 128 : 64 * 128);
-        float (&d)[BN / 2] = *reinterpret_cast<float(*)[BN / 2]>(&acc[0][0][0]);
-        wgmma_fence_regs(d);
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < kBK / El::MMA_K; ++ks) {
           const uint64_t ad = wgmma_desc_sw128(a0 + ks * (AMAJ ? 2048 : 32), kBK * 128, 1024);
           const uint64_t bd = wgmma_desc_sw128(sb_u + ks * (BMAJ ? 2048 : 32), kBK * 128, 1024);
-          if constexpr (BN == 128) wgmma_m64n128k16_f16<AMAJ, BMAJ>(d, ad, bd);
-          else                     wgmma_m64n64k16_f16<AMAJ, BMAJ>(d, ad, bd);
+          static_assert(BN == kBNHalf, "the fp16 kind runs on 256-column tiles");
+          wgmma_m64n256k16_f16<AMAJ, BMAJ>(d, ad, bd);
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(d);
+        // one k-block stays in flight, so the tensor pipe is not drained between k-blocks: this wait retires the
+        // previous k-block, whose stage the producer may now refill.  MMAs into one accumulator complete in order, so
+        // every element still sums its k16 products in k order.
+        wgmma_wait<1>();
+        if (held >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[held]);
+        }
+        held = stage;
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if constexpr (KIND == 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      }
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
       if constexpr (promote) {
 #pragma unroll
@@ -260,6 +272,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int e = 0; e < 4; ++e) { acc[i][j][e] += part[i][j][e]; part[i][j][e] = 0.f; }
       }
+    }
+
+    if constexpr (WG) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[held]);
     }
 
     // ---------------------------------------------------------------- epilogue (rows g, g + 8 of each m16 tile)
@@ -457,9 +476,9 @@ static int dispatch_major(int am, int bm, int out16, const GemmMaps& tm, const G
 
 // kind 0: A/B fp32 (tf32 tensor cores; A_lo/B_lo non-null selects the 3-pass error-compensated product)
 // kind 1: A/B fp16
-// cta_group is accepted for ABI stability and ignored (one CTA per tile on sm_90a); bn <= 64 selects 64-column
-// tiles, anything else 128.  The 3xTF32 product always runs on 64-column tiles: its promoted partial sums double the
-// accumulator registers.
+// cta_group is accepted for ABI stability and ignored (one CTA per tile on sm_90a).  The fp16 kind always runs on
+// 128 x 256 tiles (4 ring stages).  tf32: bn <= 64 selects 64-column tiles, anything else 128; the 3xTF32 product
+// always runs on 64-column tiles: its promoted partial sums double the accumulator registers.
 static int gemm_launch(int kind, const void* A, long long lda, int a_major, const void* B, long long ldb, int b_major, void* C,
                        long long ldc, int out16, int M, int N, int K, int splits, long long c_split_stride, const float* bias,
                        const float* res, long long ldres, int res_row_mod, const void* aux, long long ldaux, float* colsum_part,
@@ -486,7 +505,7 @@ static int gemm_launch(int kind, const void* A, long long lda, int a_major, cons
   B200_CHECK_ARG(!(aux && res && res_row_mod == 0), "gemm: residual and tanh' inputs cannot be combined");
   if (bn <= 0) bn = N > 64 ? 128 : 64;
   B200_CHECK_ARG(bn == 64 || bn == 128 || bn == 192 || bn == 256, "gemm: unsupported BN %d", bn);
-  bn = (bn <= 64 || A_lo) ? 64 : 128;
+  bn = kind == 1 ? kBNHalf : (bn <= 64 || A_lo) ? 64 : 128;
 
   GemmParams p;
   p.M = M; p.N = N; p.K = K;
@@ -518,10 +537,8 @@ static int gemm_launch(int kind, const void* A, long long lda, int a_major, cons
     if ((rc = opmap(&tm.b2, B_lo, ldb, N, b_major, bn))) return rc;
   }
   if (A_lo) return dispatch_major<0, 64, 1>(a_major, b_major, 0, tm, p, stream);
-  if (bn == 64) return kind == 0 ? dispatch_major<0, 64>(a_major, b_major, 0, tm, p, stream)
-                                 : dispatch_major<1, 64>(a_major, b_major, out16, tm, p, stream);
-  return kind == 0 ? dispatch_major<0, 128>(a_major, b_major, 0, tm, p, stream)
-                   : dispatch_major<1, 128>(a_major, b_major, out16, tm, p, stream);
+  if (kind == 1) return dispatch_major<1, kBNHalf>(a_major, b_major, out16, tm, p, stream);
+  return bn == 64 ? dispatch_major<0, 64>(a_major, b_major, 0, tm, p, stream) : dispatch_major<0, 128>(a_major, b_major, 0, tm, p, stream);
 }
 
 int gemm_tf32(const float* A, long long lda, int a_major, const float* B, long long ldb, int b_major, float* C,

@@ -118,13 +118,19 @@ def splitk_reduce(part: Tensor, out: Optional[Tensor] = None, alpha: Optional[Te
     return out
 
 
+# Output tile (rows, columns) of the persistent GEMM (csrc/gemm_tc.cu: kBM, kBNHalf, and the tf32 kinds' 128-column
+# tile), keyed by the k-block width in elements (64: fp16, 32: tf32): the wave model of pick_splits counts these tiles.
+GEMM_TILE = {64: (128, 256), 32: (128, 128)}
+
+
 def pick_splits(k_total: int, out_rows: int, out_cols: int, sms: int = 132, k_atom: int = 32) -> int:
     """split count for a wgrad GEMM, by a two-term cost model.  The persistent kernel runs ceil(tiles * splits / sms) waves
-    of 128 x 128 tiles (one CTA per SM), so the contraction costs flops / (peak * fill of the last wave) (to_qkv's wgrad,
-    a 2304 x 768 output: 108 tiles, 1 split = 0.82 waves, 2 splits = 1.64, 4 splits = 3.27); the partial sums cost one fp32
-    write and one read per split.  Each split contracts a multiple of one k-block (32 fp32 / 64 fp16 elements) and at least
-    256 rows."""
-    tiles = -(-out_rows // 128) * -(-out_cols // 128)
+    of GEMM_TILE[k_atom] tiles (one CTA per SM), so the contraction costs flops / (peak * fill of the last wave) (to_qkv's
+    fp16 wgrad, a 2304 x 768 output in 128 x 256 tiles: 54 tiles, 1 split = 0.41 waves, 2 splits = 0.82, 4 splits = 1.64);
+    the partial sums cost one fp32 write and one read per split.  Each split contracts a multiple of one k-block (32 fp32 /
+    64 fp16 elements) and at least 256 rows."""
+    tm, tn = GEMM_TILE[k_atom]
+    tiles = -(-out_rows // tm) * -(-out_cols // tn)
     peak = 0.99e15 if k_atom == 64 else 0.495e15       # H100 SXM dense f16 / tf32 tensor rates (data sheet)
     t_mma = 2.0 * k_total * out_rows * out_cols / peak
     best, best_t = 1, float("inf")

@@ -56,7 +56,8 @@ int b200vq_set_sm_limit(int n);
  * colsum_part (nullable, [ceil(M/16)][N], splits must be 1): receives the column sums of every 16-row group of
  * the stored C -- summed over the groups (b200vq_colsum) they are the bias gradient of the Linear whose
  * pre-activation gradient this GEMM produced (net.0, layers.py:99), without another pass over C.
- * cta_group: 1 = one CTA per 128 x bn tile, 2 = CTA pair per 256 x bn tile; bn in {0=auto,64,128,192,256}.
+ * cta_group: accepted and ignored (one CTA per tile).  bn in {0=auto,64,128,192,256} picks the tile width of the tf32
+ * kinds (64 or 128 columns); the fp16 kind always runs on 128 x 256 tiles.
  *
  * Three operand flavours:
  *   gemm_tf32   A, B fp32, tf32 MMA (10-bit mantissa; the hardware truncates, so producers round to nearest).
