@@ -2,9 +2,10 @@
 // q k^T * scale -> softmax -> . v) and the row-wise helper of its backward.
 //
 // The reference materialises and saves a [B, heads, N, N] fp32 probability tensor per layer
-// (6.4 GB at B=128, base).  Here the scores live in registers only (attention_exact.cu:
-// mma.sync flash-style forward and backward); backward recomputes them from the saved
-// log-sum-exp and needs delta = rowsum(dO * O), computed below.
+// (6.4 GB at B=128, base).  Here the scores live in registers only (attention_f16.cu: wgmma
+// kernels of the fp16 data path; attention_exact.cu: mma.sync tf32 / 3xTF32 kernels and the
+// stage-2 mask); backward recomputes them from the saved log-sum-exp and needs
+// delta = rowsum(dO * O), computed below.
 #include "common.cuh"
 
 namespace b200 {

@@ -1,19 +1,15 @@
-// Flash-style attention core on mma.sync, tf32 m16n8k8 or f16 m16n8k16 (reference enhancing/modules/stage1/layers.py:124-130 and its
+// Flash-style attention core on mma.sync tf32 m16n8k8 (reference enhancing/modules/stage1/layers.py:124-130 and its
 // autograd): the scores live in registers only, backward recomputes them from the saved log-sum-exp.
 //   PASSES == 1: one tf32 product per MMA; the softmax probabilities and dS are rounded to nearest tf32 before they
 //                re-enter the tensor core.  Serves the tf32 data path (q/k/v already tf32-rounded by the GEMM that wrote
 //                them).
-//   IN16:        the fp16 data path: fp16 q/k/v/dO staged as fp16, mma.sync m16n8k16 .f16 with ldmatrix fragments,
-//                probabilities and dS packed to fp16 pairs in registers (struct Ops below).
 //   PASSES == 3: the error-compensated 3xTF32 form  a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi  (hi = the
 //                10-bit-mantissa truncation the tensor core applies anyway, lo = x - hi, exact in fp32), split in
 //                registers: fp32-grade results (~2^-21 relative) for `precision="parity"`.
-// IN16 / OUT16 select fp16 storage of the inputs (q/k/v, dO) and of the outputs (O, dq/dk/dv).
+// OUT16 selects fp16 storage of the outputs (O, dq/dk/dv).  The fp16 data path runs on wgmma in attention_f16.cu.
 // Backward is split in two kernels so that no atomics are needed: one CTA per key tile (dK, dV) and one per
 // query tile (dQ).
 #include "common.cuh"
-
-#include <type_traits>
 
 namespace b200 {
 
@@ -35,9 +31,8 @@ __device__ __forceinline__ void mma_x(float (&c)[4], const uint32_t (&a)[4], uin
     mma_tf32(c, ah, tf32_hi(b0), tf32_hi(b1));
   }
 }
-// one element as fp32 bits, from fp32 or fp16 storage
+// one element as fp32 bits
 __device__ __forceinline__ uint32_t ldbits(const float* p) { return __float_as_uint(*p); }
-__device__ __forceinline__ uint32_t ldbits(const __half* p) { return __float_as_uint(__half2float(*p)); }
 // row pitch (elements) of a staged tile: 16 bytes of padding per row
 template <typename T, int DH> struct Pitch { static constexpr int LDS = DH + 16 / (int)sizeof(T); };
 __device__ __forceinline__ void cpa16(void* dst, const void* src, bool valid) {
@@ -129,11 +124,8 @@ __device__ __forceinline__ void store2(void* base, long long off, float a, float
   }
 }
 
-// The operand path of the kernels below.  fp32 storage: tf32 m16n8k8 (one or three passes), A fragments [DH/8][4],
-// P / dS fragments [8][4].  fp16 storage: f16 m16n8k16 with ldmatrix (B operands of both orientations straight from the
-// staged tiles), A fragments [DH/16][4], P / dS fragments packed to fp16 pairs [4][4].
-template <int DH, int PASSES, int IN16> struct Ops;
-template <int DH, int PASSES> struct Ops<DH, PASSES, 0> {
+// The operand path of the kernels below: tf32 m16n8k8 (one or three passes), A fragments [DH/8][4], P / dS fragments [8][4].
+template <int DH, int PASSES> struct Ops {
   using T = float;
   using QF = uint32_t[DH / 8][4];
   using PF = uint32_t[8][4];
@@ -150,70 +142,15 @@ template <int DH, int PASSES> struct Ops<DH, PASSES, 0> {
     acc_to_a<PASSES>(pf[nt], c0, c1, c2, c3);
   }
 };
-template <int DH> struct Ops<DH, 1, 1> {
-  using T = __half;
-  using QF = uint32_t[DH / 16][4];
-  using PF = uint32_t[4][4];
-  static constexpr int LDS = Pitch<T, DH>::LDS;
-  // A fragments of a 16 x DH row block from global memory: a0 (row g, k 2t..2t+1), a1 (row g+8), a2 / a3 (k + 8)
-  static __device__ __forceinline__ void load_a(QF& f, const T* base, long long ld, int row_lo, int nvalid, int lane) {
-    const int g = lane >> 2, t = lane & 3;
-    const int r0 = row_lo + g, r1 = row_lo + g + 8;
-    const bool ok0 = r0 < nvalid, ok1 = r1 < nvalid;
-    const T* p0 = base + (long long)(ok0 ? r0 : 0) * ld + 2 * t;
-    const T* p1 = base + (long long)(ok1 ? r1 : 0) * ld + 2 * t;
-#pragma unroll
-    for (int kc = 0; kc < DH / 16; ++kc) {
-      f[kc][0] = ok0 ? *reinterpret_cast<const uint32_t*>(p0 + kc * 16) : 0u;
-      f[kc][1] = ok1 ? *reinterpret_cast<const uint32_t*>(p1 + kc * 16) : 0u;
-      f[kc][2] = ok0 ? *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8) : 0u;
-      f[kc][3] = ok1 ? *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8) : 0u;
-    }
-  }
-  // acc[nt] += A . T^T, T a staged [64][DH] tile whose rows are the output columns: ldmatrix (no transpose) gives
-  // b0 / b1 of two n8 tiles per x4 load
-  static __device__ __forceinline__ void rows_x_tileT(float (&acc)[8][4], const QF& a, const T* Ts, int lane) {
-    const int lr = lane & 7, lj = lane >> 3;
-    const uint32_t base = smem_u32(Ts);
-#pragma unroll
-    for (int kc = 0; kc < DH / 16; ++kc)
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t v[4];
-        ldsm_x4(base + (uint32_t)(((np * 16 + (lj >> 1) * 8 + lr) * LDS + kc * 16 + (lj & 1) * 8) * 2), v);
-        mma_f16(acc[2 * np], a[kc], v[0], v[1]);
-        mma_f16(acc[2 * np + 1], a[kc], v[2], v[3]);
-      }
-  }
-  // acc[dt] += P . T, T a staged [64][DH] tile whose rows are the contraction index: ldmatrix.trans
-  static __device__ __forceinline__ void p_x_tile(float (&acc)[DH / 8][4], const PF& pf, const T* Ts, int lane) {
-    const int lr = lane & 7, lj = lane >> 3;
-    const uint32_t base = smem_u32(Ts);
-#pragma unroll
-    for (int kc = 0; kc < 4; ++kc)
-#pragma unroll
-      for (int dp = 0; dp < DH / 16; ++dp) {
-        uint32_t v[4];
-        ldsm_x4_t(base + (uint32_t)(((kc * 16 + (lj & 1) * 8 + lr) * LDS + dp * 16 + (lj >> 1) * 8) * 2), v);
-        mma_f16(acc[2 * dp], pf[kc], v[0], v[1]);
-        mma_f16(acc[2 * dp + 1], pf[kc], v[2], v[3]);
-      }
-  }
-  // accumulator tile nt (c0, c1: row g; c2, c3: row g + 8) -> half of the k16 A fragment kc = nt / 2
-  static __device__ __forceinline__ void set_p(PF& pf, int nt, float c0, float c1, float c2, float c3) {
-    pf[nt >> 1][(nt & 1) * 2] = pack_half2_sat(c0, c1);
-    pf[nt >> 1][(nt & 1) * 2 + 1] = pack_half2_sat(c2, c3);
-  }
-};
 
 // ---------------------------------------------------------------------------------------------
 // forward: grid (ceil(N/128), heads, B), 256 threads = 8 warps x 16 query rows
 // ---------------------------------------------------------------------------------------------
-template <int DH, int PASSES, int IN16, int OUT16>
+template <int DH, int PASSES, int OUT16>
 __global__ void __launch_bounds__(256)
 attn_fwd_kernel(const void* __restrict__ qkv_, void* __restrict__ out, float* __restrict__ lse, int N, int heads,
                 float scale, int cond, int round_out) {
-  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  using T = float;
   const T* qkv = static_cast<const T*>(qkv_);
   constexpr int LDS = Pitch<T, DH>::LDS;
   constexpr int TILE = 64 * LDS;
@@ -231,7 +168,7 @@ attn_fwd_kernel(const void* __restrict__ qkv_, void* __restrict__ out, float* __
   const int q0 = blockIdx.x * 128 + warp * 16;
   const float c = scale * kLog2e;
 
-  using Op = Ops<DH, PASSES, IN16>;
+  using Op = Ops<DH, PASSES>;
   typename Op::QF qf;
   Op::load_a(qf, qbase, ld, q0, N, lane);
 
@@ -328,12 +265,12 @@ attn_fwd_kernel(const void* __restrict__ qkv_, void* __restrict__ out, float* __
 // Works on transposed score tiles S^T[key, query] so that P^T / dS^T come out of the tensor
 // cores already in A-operand position for dV += P^T dO and dK += dS^T Q.
 // ---------------------------------------------------------------------------------------------
-template <int DH, int PASSES, int IN16, int OUT16>
+template <int DH, int PASSES, int OUT16>
 __global__ void __launch_bounds__(128)
 attn_bwd_dkv_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_, const float* __restrict__ lse,
                     const float* __restrict__ delta, void* __restrict__ dqkv, const float* __restrict__ out_scale, int N,
                     int heads, float scale, int cond, int round_out) {
-  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  using T = float;
   const T* qkv = static_cast<const T*>(qkv_);
   const T* dout = static_cast<const T*>(dout_);
   constexpr int LDS = Pitch<T, DH>::LDS;
@@ -355,7 +292,7 @@ attn_bwd_dkv_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout
   const int k0 = blockIdx.x * 64 + warp * 16;
   const float c = scale * kLog2e;
 
-  using Op = Ops<DH, PASSES, IN16>;
+  using Op = Ops<DH, PASSES>;
   typename Op::QF kf, vf;
   Op::load_a(kf, qbase + inner, ld, k0, N, lane);
   Op::load_a(vf, qbase + 2 * inner, ld, k0, N, lane);
@@ -440,12 +377,12 @@ attn_bwd_dkv_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout
 // ---------------------------------------------------------------------------------------------
 // backward, query side: grid (ceil(N/64), heads, B), 128 threads = 4 warps x 16 queries
 // ---------------------------------------------------------------------------------------------
-template <int DH, int PASSES, int IN16, int OUT16>
+template <int DH, int PASSES, int OUT16>
 __global__ void __launch_bounds__(128)
 attn_bwd_dq_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_, const float* __restrict__ lse,
                    const float* __restrict__ delta, void* __restrict__ dqkv, const float* __restrict__ out_scale, int N,
                    int heads, float scale, int cond, int round_out) {
-  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  using T = float;
   const T* qkv = static_cast<const T*>(qkv_);
   const T* dout = static_cast<const T*>(dout_);
   constexpr int LDS = Pitch<T, DH>::LDS;
@@ -470,7 +407,7 @@ attn_bwd_dq_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_
   const float lse0 = r0 < N ? lb[r0] * kLog2e : INFINITY, lse1 = r1 < N ? lb[r1] * kLog2e : INFINITY;
   const float e0 = r0 < N ? eb[r0] : 0.f, e1 = r1 < N ? eb[r1] : 0.f;
 
-  using Op = Ops<DH, PASSES, IN16>;
+  using Op = Ops<DH, PASSES>;
   typename Op::QF qf, dof;
   Op::load_a(qf, qbase, ld, q0, N, lane);
   Op::load_a(dof, dobase, inner, q0, N, lane);
@@ -521,26 +458,26 @@ attn_bwd_dq_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_
 
 
 // ---------------------------------------------------------------------------------------------
-template <int DH, int PASSES, int IN16, int OUT16>
+template <int DH, int PASSES, int OUT16>
 static int fwd_launch(const void* qkv, void* out, float* lse, int B, int N, int heads, float scale, int cond, int round_out,
                       cudaStream_t s) {
-  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  using T = float;
   constexpr size_t smem = 4 * 64 * Pitch<T, DH>::LDS * sizeof(T);
-  auto kern = attn_fwd_kernel<DH, PASSES, IN16, OUT16>;
+  auto kern = attn_fwd_kernel<DH, PASSES, OUT16>;
   B200_CONFIGURE_SMEM_ONCE(kern, smem);
   kern<<<dim3((N + 127) / 128, heads, B), 256, smem, s>>>(qkv, out, lse, N, heads, scale, cond, round_out);
   B200_LAUNCH_OK("attn_fwd_kernel");
   return 0;
 }
 
-template <int DH, int PASSES, int IN16, int OUT16>
+template <int DH, int PASSES, int OUT16>
 static int bwd_launch(const void* qkv, const void* dout, const float* lse, const float* delta, void* dqkv, const float* out_scale,
                       int B, int N, int heads, float scale, int cond, int round_out, cudaStream_t s) {
-  using T = typename std::conditional<IN16 != 0, __half, float>::type;
+  using T = float;
   constexpr size_t smem_kv = 4 * 64 * Pitch<T, DH>::LDS * sizeof(T) + 256 * sizeof(float);
   constexpr size_t smem_q = 4 * 64 * Pitch<T, DH>::LDS * sizeof(T);
-  auto k1 = attn_bwd_dkv_kernel<DH, PASSES, IN16, OUT16>;
-  auto k2 = attn_bwd_dq_kernel<DH, PASSES, IN16, OUT16>;
+  auto k1 = attn_bwd_dkv_kernel<DH, PASSES, OUT16>;
+  auto k2 = attn_bwd_dq_kernel<DH, PASSES, OUT16>;
   B200_CONFIGURE_SMEM_ONCE(k1, smem_kv);
   B200_CONFIGURE_SMEM_ONCE(k2, smem_q);
   const dim3 grid((N + 63) / 64, heads, B);
@@ -568,8 +505,8 @@ static int check_problem(const void* qkv, int B, int N, int heads, int dh, int c
 int attention_exact_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
                             int cond_len, cudaStream_t stream) {
   if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
-  if (dh == 64) return fwd_launch<64, 3, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
-  return fwd_launch<32, 3, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
+  if (dh == 64) return fwd_launch<64, 3, 0>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
+  return fwd_launch<32, 3, 0>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
 }
 
 int attention_exact_backward(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv, float* delta,
@@ -577,18 +514,18 @@ int attention_exact_backward(const float* qkv, const float* out, const float* ls
   if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
   int rc = attention_delta(out, 0, dout, 0, delta, B, N, heads, dh, stream);
   if (rc) return rc;
-  if (dh == 64) return bwd_launch<64, 3, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
-  return bwd_launch<32, 3, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
+  if (dh == 64) return bwd_launch<64, 3, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
+  return bwd_launch<32, 3, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
 }
 
 // tf32 core: fp32 q/k/v (tf32-rounded by the GEMM that wrote them); O in fp32 (optionally tf32-rounded) or fp16
 int attention_forward_tc(const float* qkv, void* out, int out_half, float* lse, int B, int N, int heads, int dh, float scale,
                          int round_out, int cond_len, cudaStream_t stream) {
   if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
-  if (dh == 64) return out_half ? fwd_launch<64, 1, 0, 1>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
-                                : fwd_launch<64, 1, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
-  return out_half ? fwd_launch<32, 1, 0, 1>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
-                  : fwd_launch<32, 1, 0, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
+  if (dh == 64) return out_half ? fwd_launch<64, 1, 1>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
+                                : fwd_launch<64, 1, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
+  return out_half ? fwd_launch<32, 1, 1>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
+                  : fwd_launch<32, 1, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
 }
 
 // delta must already hold rowsum(dO * O).  dqkv fp32 (optionally tf32-rounded) or, with out_half, fp16(dqkv * out_scale[0]).
@@ -597,32 +534,10 @@ int attention_backward_tc(const float* qkv, const float* dout, const float* lse,
                           cudaStream_t stream) {
   if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dout) & 15) == 0, "attention: dout must be 16-byte aligned");
-  if (dh == 64) return out_half ? bwd_launch<64, 1, 0, 1>(qkv, dout, lse, delta, dqkv, out_scale, B, N, heads, scale, cond_len, 0, stream)
-                                : bwd_launch<64, 1, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, round_out, stream);
-  return out_half ? bwd_launch<32, 1, 0, 1>(qkv, dout, lse, delta, dqkv, out_scale, B, N, heads, scale, cond_len, 0, stream)
-                  : bwd_launch<32, 1, 0, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, round_out, stream);
-}
-
-// fp16 core (dim_head 64): q/k/v fp16 as the to_qkv GEMM stores them, O fp16.  Backward: dO fp16 carrying the power-of-two
-// gradient scale S of the backward segment (functional.py); delta, dS and the stored fp16 dq / dk / dv carry S too --
-// everything is linear in dO, nothing is rescaled here.
-int attention_f16_forward(const void* qkv, void* out, float* lse, int B, int N, int heads, int dh, float scale, cudaStream_t stream) {
-  B200_CHECK_ARG(dh == 64, "attention_f16: dim_head must be 64 (got %d); other head sizes use the tf32 core", dh);
-  if (int rc = check_problem(qkv, B, N, heads, dh, -1)) return rc;
-  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 15) == 0, "attention: out must be 16-byte aligned");
-  return fwd_launch<64, 1, 1, 1>(qkv, out, lse, B, N, heads, scale, -1, 0, stream);
-}
-
-int attention_f16_backward(const void* qkv, const void* out, const float* lse, const void* dout, void* dqkv, float* delta, int B, int N,
-                           int heads, int dh, float scale, cudaStream_t stream) {
-  B200_CHECK_ARG(dh == 64, "attention_f16: dim_head must be 64 (got %d)", dh);
-  if (int rc = check_problem(qkv, B, N, heads, dh, -1)) return rc;
-  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dout) & 15) == 0 && (reinterpret_cast<uintptr_t>(dqkv) & 15) == 0 &&
-                     (reinterpret_cast<uintptr_t>(out) & 15) == 0,
-                 "attention: qkv/out/dout/dqkv must be 16-byte aligned");
-  int rc = attention_delta(out, 1, dout, 1, delta, B, N, heads, dh, stream);
-  if (rc) return rc;
-  return bwd_launch<64, 1, 1, 1>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, -1, 0, stream);
+  if (dh == 64) return out_half ? bwd_launch<64, 1, 1>(qkv, dout, lse, delta, dqkv, out_scale, B, N, heads, scale, cond_len, 0, stream)
+                                : bwd_launch<64, 1, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, round_out, stream);
+  return out_half ? bwd_launch<32, 1, 1>(qkv, dout, lse, delta, dqkv, out_scale, B, N, heads, scale, cond_len, 0, stream)
+                  : bwd_launch<32, 1, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, round_out, stream);
 }
 
 }  // namespace b200
