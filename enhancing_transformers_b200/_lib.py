@@ -38,6 +38,8 @@ _SIGNATURES = {
     "b200vq_vq_workspace_bytes": (c_sz, [c_i, c_i, c_i]),
     "b200vq_vq_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_fl, c_i, c_f, c_sz, c_f]),
     "b200vq_vq_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_fl, c_i, c_f]),
+    "b200vq_vq_bwd_deterministic_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i]),
+    "b200vq_vq_bwd_deterministic": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_fl, c_i, c_f, c_sz, c_f]),
     "b200vq_vq_embed": (c_i, [c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_patchify": (c_i, [c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_unpatchify": (c_i, [c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
@@ -59,6 +61,8 @@ _SIGNATURES = {
     "b200vq_sqrelu": (c_i, [c_f, c_f, c_f, c_ll, c_i, c_i, c_f]),
     "b200vq_token_embed_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_token_embed_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
+    "b200vq_token_embed_bwd_deterministic_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i, c_i, c_i]),
+    "b200vq_token_embed_bwd_deterministic": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_f, c_sz, c_f]),
     "b200vq_copy_rows": (c_i, [c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_decode_attention": (c_i, [c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_fl, c_f]),
 }

@@ -84,6 +84,9 @@ int vq_forward(const float*, const float*, float*, long long*, float*, int, int,
 int vq_backward(const float*, const float*, const long long*, const float*, const float*, float*, float*, int, int, int, int,
                 int, float, int, cudaStream_t);
 int vq_embed(const float*, const long long*, float*, int, int, int, int, int, cudaStream_t);
+size_t vq_bwd_deterministic_workspace_bytes(int, int, int, int);
+int vq_backward_deterministic(const float*, const float*, const long long*, const float*, const float*, float*, float*, int, int, int,
+                              int, int, float, int, void*, size_t, cudaStream_t);
 int patchify(const float*, float*, int, int, int, int, int, int, int, cudaStream_t);
 int unpatchify(const float*, const float*, float*, int, int, int, int, int, int, cudaStream_t);
 size_t colsum_workspace_bytes(int);
@@ -104,6 +107,9 @@ int token_embed_forward(const long long*, const long long*, const float*, const 
                         int, int, int, int, cudaStream_t);
 int token_embed_backward(const long long*, const long long*, const float*, float*, float*, float*, float*, int, int, int, int, int,
                          int, cudaStream_t);
+size_t token_embed_bwd_deterministic_workspace_bytes(int, int, int, int, int, int);
+int token_embed_backward_deterministic(const long long*, const long long*, const float*, float*, float*, float*, float*, int, int, int,
+                                       int, int, int, void*, size_t, cudaStream_t);
 int copy_rows(const float*, float*, int, int, int, int, int, int, int, cudaStream_t);
 int decode_attention(const float*, float*, float*, float*, int, int, int, int, int, float, cudaStream_t);
 
@@ -201,6 +207,15 @@ int b200vq_vq_bwd(const float* z, const float* E, const long long* idx, const fl
                   float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm, void* stream) {
   return vq_backward(z, E, idx, g_out, g_loss, gz, gE, M, K, D, depth, residual, beta, use_norm, S(stream));
 }
+size_t b200vq_vq_bwd_deterministic_workspace_bytes(int M, int K, int D, int depth) {
+  return vq_bwd_deterministic_workspace_bytes(M, K, D, depth);
+}
+int b200vq_vq_bwd_deterministic(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss,
+                                float* gz, float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm,
+                                void* workspace, size_t ws_bytes, void* stream) {
+  return vq_backward_deterministic(z, E, idx, g_out, g_loss, gz, gE, M, K, D, depth, residual, beta, use_norm, workspace, ws_bytes,
+                                   S(stream));
+}
 int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
                     void* stream) {
   return vq_embed(E, codes, out, M, K, D, depth, use_norm, S(stream));
@@ -258,6 +273,15 @@ int b200vq_token_embed_fwd(const long long* conds, const long long* codes, const
 int b200vq_token_embed_bwd(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c, float* gWi,
                            float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* stream) {
   return token_embed_backward(conds, codes, g, gWc, gpos_c, gWi, gpos_i, B, Tc, Ti, C, Vc, Vi, S(stream));
+}
+size_t b200vq_token_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int Ti, int C, int Vc, int Vi) {
+  return token_embed_bwd_deterministic_workspace_bytes(B, Tc, Ti, C, Vc, Vi);
+}
+int b200vq_token_embed_bwd_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                         float* gWi, float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* workspace,
+                                         size_t ws_bytes, void* stream) {
+  return token_embed_backward_deterministic(conds, codes, g, gWc, gpos_c, gWi, gpos_i, B, Tc, Ti, C, Vc, Vi, workspace, ws_bytes,
+                                            S(stream));
 }
 int b200vq_copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, int off_src, int off_dst, int n, int C,
                      void* stream) {

@@ -7,7 +7,10 @@
 //   copy_rows    x[:, a:b] row windows (logits are taken at positions cond-1 .. T-2)          (layers.py:210)
 //   decode_attention  one query per (batch, head) against the KV cache                        (layers.py:76-81, sampling)
 // All HBM-bound streams: float4 grid-stride loops, no shared-memory staging needed (every element is read once).
+// token_embed's backward scatters the table gradients with float atomics, or, on request, sums them in a fixed order
+// through scatter_det.cu (bit-reproducible).
 #include "common.cuh"
+#include "scatter_det.cuh"
 
 namespace b200 {
 
@@ -144,6 +147,21 @@ token_embed_bwd_kernel(const long long* __restrict__ conds, const long long* __r
   }
 }
 
+// gpos_c / gpos_i alone, with token_embed_bwd_kernel's arithmetic (one thread walks the batch); the deterministic backward
+// takes gWc / gWi from scatter_rows_det.  Grid from the shape: one thread per (t, c).
+__global__ void __launch_bounds__(256)
+token_embed_pos_bwd_kernel(const float* __restrict__ g, float* __restrict__ gpos_c, float* __restrict__ gpos_i, int B, int Tc, int Ti,
+                           int C) {
+  const int T = Tc + Ti;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)T * C) return;
+  const int t = (int)(i / C), c = (int)(i - (long long)t * C);
+  float acc = 0.f;
+  for (int b = 0; b < B; ++b) acc += g[((long long)b * T + t) * C + c];
+  if (t < Tc) gpos_c[(long long)t * C + c] = acc;
+  else        gpos_i[(long long)(t - Tc) * C + c] = acc;
+}
+
 // dst[b, t] = (off_dst <= t < off_dst + n) ? src[b, t - off_dst + off_src] : 0      (dst [B, T_dst, C], src [B, T_src, C])
 __global__ void __launch_bounds__(256)
 copy_rows_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int T_src, int T_dst, int off_src, int off_dst, int n,
@@ -266,6 +284,34 @@ int token_embed_backward(const long long* conds, const long long* codes, const f
   token_embed_bwd_kernel<<<s2_grid((long long)(Tc + Ti) * C, 256), 256, 0, stream>>>(conds, codes, g, gWc, gpos_c, gWi, gpos_i, B, Tc,
                                                                                     Ti, C, Vc, Vi);
   B200_LAUNCH_OK("token_embed_bwd_kernel");
+  return 0;
+}
+
+// one scatter workspace, reused by the two tables in turn
+size_t token_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int Ti, int C, int Vc, int Vi) {
+  if (B <= 0 || Tc < 0 || Ti < 0 || C <= 0) return 0;
+  const size_t wc = Vc > 0 ? scatter_det_workspace_bytes((long long)B * Tc, Vc, C, kScatterRunToken) : 0;
+  const size_t wi = Vi > 0 ? scatter_det_workspace_bytes((long long)B * Ti, Vi, C, kScatterRunToken) : 0;
+  return wc > wi ? wc : wi;
+}
+
+int token_embed_backward_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                       float* gWi, float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* workspace,
+                                       size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(B > 0 && Tc >= 0 && Ti >= 0 && Tc + Ti > 0 && C > 0, "token_embed: bad shape B=%d Tc=%d Ti=%d C=%d", B, Tc, Ti, C);
+  B200_CHECK_ARG(Vc > 0 && Vi > 0, "token_embed: vocabulary sizes must be positive (Vc=%d Vi=%d)", Vc, Vi);
+  B200_CHECK_ARG((long long)B * (Tc + Ti) <= (1LL << 30), "token_embed: too many tokens");
+  B200_CHECK_ARG(g && gWc && gWi && (Tc == 0 || (conds && gpos_c)) && (Ti == 0 || (codes && gpos_i)) && workspace,
+                 "token_embed_bwd_deterministic: null pointer argument");
+  B200_CHECK_ARG(ws_bytes >= token_embed_bwd_deterministic_workspace_bytes(B, Tc, Ti, C, Vc, Vi),
+                 "token_embed_bwd_deterministic: workspace too small");
+  const long long T = Tc + Ti;
+  int rc = scatter_rows_det<kScatterRunToken>(conds, (long long)B * Tc, Vc, g, Tc, T, 0, C, gWc, workspace, ws_bytes, stream);
+  if (rc) return rc;
+  rc = scatter_rows_det<kScatterRunToken>(codes, (long long)B * Ti, Vi, g, Ti, T, Tc, C, gWi, workspace, ws_bytes, stream);
+  if (rc) return rc;
+  token_embed_pos_bwd_kernel<<<(unsigned)((T * C + 255) / 256), 256, 0, stream>>>(g, gpos_c, gpos_i, B, Tc, Ti, C);
+  B200_LAUNCH_OK("token_embed_pos_bwd_kernel");
   return 0;
 }
 

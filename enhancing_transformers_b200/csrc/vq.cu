@@ -9,8 +9,11 @@
 //             depth loop (:42-57) runs inside the kernel.  The [tokens, n_embed] distance
 //             matrix the reference materialises never exists.
 //   vq_loss : deterministic reduction of the per-CTA partial sums into the scalar loss.
-//   vq_bwd  : closed-form gradients (see oracle/vitvq_oracle.py:vq_backward_np).
+//   vq_bwd  : closed-form gradients (see oracle/vitvq_oracle.py:vq_backward_np).  The codebook gradient is scattered with
+//             float atomics (vq_bwd_kernel) or, on request, stored per entry and summed in a fixed order
+//             (vq_bwd_contrib_kernel + scatter_det.cu): bit-reproducible.
 #include "common.cuh"
+#include "scatter_det.cuh"
 
 namespace b200 {
 
@@ -304,6 +307,71 @@ __device__ __forceinline__ void vq_scatter(VqBwdTable& tb, float* __restrict__ g
   atomicAdd(dst + 0, v.x); atomicAdd(dst + 1, v.y); atomicAdd(dst + 2, v.z); atomicAdd(dst + 3, v.w);
 }
 
+// The per-token closed-form gradients of the backward, shared by the atomic and the deterministic kernel so both run the
+// same arithmetic: returns g_z's 4-float `part` of token tk and hands every codebook contribution to
+// emit(t, code, value) -- the plain quantiser once (t = 0), the residual one per depth step, deepest first.  A dead
+// token (past M, kept so that 8-lane groups stay whole) emits zeros.
+template <class Emit>
+__device__ __forceinline__ float4 vq_bwd_token(const float* __restrict__ z, const float* __restrict__ E,
+                                               const long long* __restrict__ idx, const float* __restrict__ g_out,
+                                               float g_loss, int tk, bool live, int part, int M, int depth, int residual,
+                                               float beta, int use_norm, Emit&& emit) {
+  const float c = 2.f / ((float)M * (float)kVqD);
+  const float4 zv = *reinterpret_cast<const float4*>(z + (size_t)tk * kVqD + part * 4);
+  float4 go = g_out ? *reinterpret_cast<const float4*>(g_out + (size_t)tk * kVqD + part * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+  if (!residual) {
+    const long long code = idx[tk];
+    const float4 e = *reinterpret_cast<const float4*>(E + (size_t)code * kVqD + part * 4);
+    float nz, ne;
+    const float4 zn = normalize8(zv, nz, use_norm);
+    const float4 qn = normalize8(e, ne, use_norm);
+    const float4 dzq = make_float4(zn.x - qn.x, zn.y - qn.y, zn.z - qn.z, zn.w - qn.w);
+    const float4 jz = norm_jt8(zn, nz, dzq, use_norm);
+    const float sz = g_loss * beta * c;
+    go.x += sz * jz.x; go.y += sz * jz.y; go.z += sz * jz.z; go.w += sz * jz.w;
+    const float4 dqz = make_float4(-dzq.x, -dzq.y, -dzq.z, -dzq.w);
+    const float4 je = norm_jt8(qn, ne, dqz, use_norm);
+    const float se = live ? g_loss * c : 0.f;
+    emit(0, code, make_float4(se * je.x, se * je.y, se * je.z, se * je.w));
+  } else {
+    const float gl = g_loss / (float)depth;
+    float4 r = zv;
+    float4 gq[kVqMaxDepth], gr[kVqMaxDepth], qh[kVqMaxDepth];
+    float qn_norm[kVqMaxDepth];
+#pragma unroll
+    for (int t = 0; t < kVqMaxDepth; ++t) {
+      if (t < depth) {
+        const long long code = idx[(size_t)tk * depth + t];
+        const float4 e = *reinterpret_cast<const float4*>(E + (size_t)code * kVqD + part * 4);
+        float nr, ne;
+        const float4 rn = normalize8(r, nr, use_norm);
+        const float4 qn = normalize8(e, ne, use_norm);
+        qh[t] = qn; qn_norm[t] = ne;
+        const float s1 = gl * c;
+        gq[t] = make_float4(s1 * (qn.x - rn.x), s1 * (qn.y - rn.y), s1 * (qn.z - rn.z), s1 * (qn.w - rn.w));
+        const float4 d = make_float4(rn.x - qn.x, rn.y - qn.y, rn.z - qn.z, rn.w - qn.w);
+        const float4 j = norm_jt8(rn, nr, d, use_norm);
+        const float s2 = gl * beta * c;
+        gr[t] = make_float4(s2 * j.x, s2 * j.y, s2 * j.z, s2 * j.w);
+        r.x -= qn.x; r.y -= qn.y; r.z -= qn.z; r.w -= qn.w;
+      }
+    }
+    float4 suffix = make_float4(0.f, 0.f, 0.f, 0.f);   // sum_{t > s} gr[t]
+#pragma unroll
+    for (int s = kVqMaxDepth - 1; s >= 0; --s) {
+      if (s < depth) {
+        const float4 tot = make_float4(gq[s].x - suffix.x, gq[s].y - suffix.y, gq[s].z - suffix.z, gq[s].w - suffix.w);
+        float4 je = norm_jt8(qh[s], qn_norm[s], tot, use_norm);
+        if (!live) je = make_float4(0.f, 0.f, 0.f, 0.f);
+        const long long code = idx[(size_t)tk * depth + s];
+        emit(s, code, je);
+        suffix.x += gr[s].x; suffix.y += gr[s].y; suffix.z += gr[s].z; suffix.w += gr[s].w;
+      }
+    }
+  }
+  return go;
+}
+
 // gz [M,32] (written), gE [K,32] (atomically accumulated; caller zero-fills)
 __global__ void __launch_bounds__(kVqBwdThreads)
 vq_bwd_kernel(const float* __restrict__ z, const float* __restrict__ E, const long long* __restrict__ idx,
@@ -315,64 +383,13 @@ vq_bwd_kernel(const float* __restrict__ z, const float* __restrict__ E, const lo
   __syncthreads();
   const int part = threadIdx.x & 7;
   const float g_loss = g_loss_ptr ? *g_loss_ptr : 0.f;
-  const float c = 2.f / ((float)M * (float)kVqD);
   // 32 tokens per CTA pass; M % 4 == 0 (host) keeps every 8-lane group and every warp uniform
   for (int tok0 = blockIdx.x * (kVqBwdThreads / 8); tok0 < M; tok0 += gridDim.x * (kVqBwdThreads / 8)) {
     const int tok = tok0 + (threadIdx.x >> 3);
     const bool live = tok < M;
     const int tk = live ? tok : 0;
-    const float4 zv = *reinterpret_cast<const float4*>(z + (size_t)tk * kVqD + part * 4);
-    float4 go = g_out ? *reinterpret_cast<const float4*>(g_out + (size_t)tk * kVqD + part * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!residual) {
-      const long long code = idx[tk];
-      const float4 e = *reinterpret_cast<const float4*>(E + (size_t)code * kVqD + part * 4);
-      float nz, ne;
-      const float4 zn = normalize8(zv, nz, use_norm);
-      const float4 qn = normalize8(e, ne, use_norm);
-      const float4 dzq = make_float4(zn.x - qn.x, zn.y - qn.y, zn.z - qn.z, zn.w - qn.w);
-      const float4 jz = norm_jt8(zn, nz, dzq, use_norm);
-      const float sz = g_loss * beta * c;
-      go.x += sz * jz.x; go.y += sz * jz.y; go.z += sz * jz.z; go.w += sz * jz.w;
-      const float4 dqz = make_float4(-dzq.x, -dzq.y, -dzq.z, -dzq.w);
-      const float4 je = norm_jt8(qn, ne, dqz, use_norm);
-      const float se = live ? g_loss * c : 0.f;
-      vq_scatter(tb, gE, code, part, make_float4(se * je.x, se * je.y, se * je.z, se * je.w));
-    } else {
-      const float gl = g_loss / (float)depth;
-      float4 r = zv;
-      float4 gq[kVqMaxDepth], gr[kVqMaxDepth], qh[kVqMaxDepth];
-      float qn_norm[kVqMaxDepth];
-#pragma unroll
-      for (int t = 0; t < kVqMaxDepth; ++t) {
-        if (t < depth) {
-          const long long code = idx[(size_t)tk * depth + t];
-          const float4 e = *reinterpret_cast<const float4*>(E + (size_t)code * kVqD + part * 4);
-          float nr, ne;
-          const float4 rn = normalize8(r, nr, use_norm);
-          const float4 qn = normalize8(e, ne, use_norm);
-          qh[t] = qn; qn_norm[t] = ne;
-          const float s1 = gl * c;
-          gq[t] = make_float4(s1 * (qn.x - rn.x), s1 * (qn.y - rn.y), s1 * (qn.z - rn.z), s1 * (qn.w - rn.w));
-          const float4 d = make_float4(rn.x - qn.x, rn.y - qn.y, rn.z - qn.z, rn.w - qn.w);
-          const float4 j = norm_jt8(rn, nr, d, use_norm);
-          const float s2 = gl * beta * c;
-          gr[t] = make_float4(s2 * j.x, s2 * j.y, s2 * j.z, s2 * j.w);
-          r.x -= qn.x; r.y -= qn.y; r.z -= qn.z; r.w -= qn.w;
-        }
-      }
-      float4 suffix = make_float4(0.f, 0.f, 0.f, 0.f);   // sum_{t > s} gr[t]
-#pragma unroll
-      for (int s = kVqMaxDepth - 1; s >= 0; --s) {
-        if (s < depth) {
-          const float4 tot = make_float4(gq[s].x - suffix.x, gq[s].y - suffix.y, gq[s].z - suffix.z, gq[s].w - suffix.w);
-          float4 je = norm_jt8(qh[s], qn_norm[s], tot, use_norm);
-          if (!live) je = make_float4(0.f, 0.f, 0.f, 0.f);
-          const long long code = idx[(size_t)tk * depth + s];
-          vq_scatter(tb, gE, code, part, je);
-          suffix.x += gr[s].x; suffix.y += gr[s].y; suffix.z += gr[s].z; suffix.w += gr[s].w;
-        }
-      }
-    }
+    const float4 go = vq_bwd_token(z, E, idx, g_out, g_loss, tk, live, part, M, depth, residual, beta, use_norm,
+                                   [&](int, long long code, const float4& v) { vq_scatter(tb, gE, code, part, v); });
     if (live) *reinterpret_cast<float4*>(gz + (size_t)tok * kVqD + part * 4) = go;
   }
   __syncthreads();
@@ -385,6 +402,26 @@ vq_bwd_kernel(const float* __restrict__ z, const float* __restrict__ E, const lo
       if (v != 0.f) atomicAdd(gE + (size_t)key * kVqD + (i % kVqD), v);
     }
   }
+}
+
+// Deterministic backward, first half: the same per-token work as vq_bwd_kernel, one pass of 32 tokens per CTA.  Instead of
+// scattering, entry m * depth + t (m for the plain quantiser: the layout of idx) stores its codebook contribution in
+// contrib [entries, 32]; scatter_rows_det then sums them into gE in a fixed order.
+__global__ void __launch_bounds__(kVqBwdThreads)
+vq_bwd_contrib_kernel(const float* __restrict__ z, const float* __restrict__ E, const long long* __restrict__ idx,
+                      const float* __restrict__ g_out, const float* __restrict__ g_loss_ptr, float* __restrict__ gz,
+                      float* __restrict__ contrib, int M, int depth, int residual, float beta, int use_norm) {
+  const int part = threadIdx.x & 7;
+  const float g_loss = g_loss_ptr ? *g_loss_ptr : 0.f;
+  const int tok = blockIdx.x * (kVqBwdThreads / 8) + (threadIdx.x >> 3);
+  const bool live = tok < M;
+  const int tk = live ? tok : 0;
+  const float4 go = vq_bwd_token(z, E, idx, g_out, g_loss, tk, live, part, M, depth, residual, beta, use_norm,
+                                 [&](int t, long long, const float4& v) {
+                                   const size_t entry = residual ? (size_t)tk * depth + t : (size_t)tk;
+                                   if (live) *reinterpret_cast<float4*>(contrib + entry * kVqD + part * 4) = v;
+                                 });
+  if (live) *reinterpret_cast<float4*>(gz + (size_t)tok * kVqD + part * 4) = go;
 }
 
 // decode_codes support (vitvqgan.py:81-86): out[m] = sum_t normalize(E[code[m,t]])
@@ -447,6 +484,32 @@ int vq_backward(const float* z, const float* E, const long long* idx, const floa
   vq_bwd_kernel<<<blocks, kVqBwdThreads, 0, stream>>>(z, E, idx, g_out, g_loss, gz, gE, M, K, depth, residual, beta, use_norm);
   B200_LAUNCH_OK("vq_bwd_kernel");
   return 0;
+}
+
+// contributions [M * depth, 32], then the scatter's own scratch
+size_t vq_bwd_deterministic_workspace_bytes(int M, int K, int D, int depth) {
+  if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || D != kVqD) return 0;
+  const long long n = (long long)M * depth;
+  const size_t contrib = ((size_t)n * kVqD * sizeof(float) + 255) & ~size_t(255);
+  return contrib + scatter_det_workspace_bytes(n, K, kVqD, kScatterRunVq);
+}
+
+int vq_backward_deterministic(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss,
+                              float* gz, float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm,
+                              void* workspace, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(M > 0 && M % 4 == 0 && K > 0 && K % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
+  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
+  B200_CHECK_ARG(z && E && idx && gz && gE && workspace, "vq_bwd_deterministic: null pointer argument");
+  B200_CHECK_ARG(ws_bytes >= vq_bwd_deterministic_workspace_bytes(M, K, D, depth), "vq_bwd_deterministic: workspace too small");
+  const long long n = residual ? (long long)M * depth : M;   // entries: the plain quantiser reads idx[m]
+  float* contrib = static_cast<float*>(workspace);
+  const size_t contrib_bytes = ((size_t)M * depth * kVqD * sizeof(float) + 255) & ~size_t(255);
+  vq_bwd_contrib_kernel<<<(M + 31) / 32, kVqBwdThreads, 0, stream>>>(z, E, idx, g_out, g_loss, gz, contrib, M, depth, residual,
+                                                                      beta, use_norm);
+  B200_LAUNCH_OK("vq_bwd_contrib_kernel");
+  return scatter_rows_det<kScatterRunVq>(idx, n, K, contrib, n, 0, 0, kVqD, gE, static_cast<uint8_t*>(workspace) + contrib_bytes,
+                                         ws_bytes - contrib_bytes, stream);
 }
 
 int vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,

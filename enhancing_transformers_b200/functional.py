@@ -184,6 +184,14 @@ LAYER_PARAMS = 11
 # 1e-3 tolerance is measured on), and the extra passes cost ~1 ms per 250 ms step.
 PRECISE_IO = os.environ.get("B200VQ_PRECISE_IO", "1") != "0"
 ATTENTION_F16 = os.environ.get("B200VQ_ATTENTION_F16", "1") != "0"   # fp16 mode: fp16-operand attention core for dim_head 64
+# Bit-reproducible backward on request: the codebook and token-embedding gradients are then summed in a fixed order
+# instead of with float atomics (every other kernel of the path is deterministic already).  B200VQ_DETERMINISTIC=1, or
+# torch.use_deterministic_algorithms(True), checked when the backward runs.
+DETERMINISTIC = os.environ.get("B200VQ_DETERMINISTIC", "0") == "1"
+
+
+def deterministic() -> bool:
+    return DETERMINISTIC or torch.are_deterministic_algorithms_enabled()
 
 
 def f16_supported(dim: int, inner: int, mlp: int) -> bool:
@@ -630,5 +638,6 @@ class VectorQuantizeFn(torch.autograd.Function):
             g_out = g_out.contiguous()
         if g_loss is not None:
             g_loss = g_loss.contiguous()
-        gz, gE = ops.vq_bwd(z, E, idx, g_out, g_loss, residual, beta, use_norm)
+        bwd = ops.vq_bwd_deterministic if deterministic() else ops.vq_bwd
+        gz, gE = bwd(z, E, idx, g_out, g_loss, residual, beta, use_norm)
         return gz, gE, None, None, None, None

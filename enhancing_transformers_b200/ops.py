@@ -309,6 +309,25 @@ def vq_bwd(z: Tensor, E: Tensor, idx: Tensor, g_out: Optional[Tensor], g_loss: O
     return gz, gE
 
 
+def vq_bwd_deterministic(z: Tensor, E: Tensor, idx: Tensor, g_out: Optional[Tensor], g_loss: Optional[Tensor], residual: bool,
+                         beta: float, use_norm: bool = True) -> Tuple[Tensor, Tensor]:
+    """vq_bwd with a bit-reproducible codebook gradient: gz is vq_bwd's bit for bit, gE is summed in an order that
+    depends only on idx and the shape (no float atomics)"""
+    _req(z, "z"); _req(E, "embedding.weight"); _req(idx, "idx", torch.int64); _req(g_out, "g_out"); _req(g_loss, "g_loss")
+    K, D = E.shape
+    M = z.numel() // D
+    depth = idx.shape[-1] if idx.dim() == 2 else 1
+    L = _lib.lib()
+    ws_bytes = L.b200vq_vq_bwd_deterministic_workspace_bytes(M, K, D, depth)
+    ws = torch.empty(max(ws_bytes, 1), device=z.device, dtype=torch.uint8)
+    gz = torch.empty_like(z)
+    gE = torch.empty_like(E)
+    _lib.check(L.b200vq_vq_bwd_deterministic(_p(z), _p(E), _p(idx), _p(g_out), _p(g_loss), _p(gz), _p(gE), M, K, D, depth,
+                                             int(residual), float(beta), int(use_norm), _p(ws), ws_bytes, _stream()),
+               "vq_bwd_deterministic")
+    return gz, gE
+
+
 def vq_embed(E: Tensor, codes: Tensor, depth: int, use_norm: bool = True) -> Tensor:
     _req(E, "embedding.weight"); _req(codes, "codes", torch.int64)
     K, D = E.shape
@@ -447,6 +466,25 @@ def token_embed_bwd(conds: Tensor, codes: Tensor, g: Tensor, Vc: int, Vi: int) -
     gpi = torch.empty(Ti, C, device=g.device, dtype=torch.float32)
     _lib.check(_lib.lib().b200vq_token_embed_bwd(_p(conds), _p(codes), _p(g), _p(gWc), _p(gpc), _p(gWi), _p(gpi), B, Tc, Ti, C, Vc, Vi,
                                                  _stream()), "token_embed_bwd")
+    return gWc, gpc, gWi, gpi
+
+
+def token_embed_bwd_deterministic(conds: Tensor, codes: Tensor, g: Tensor, Vc: int, Vi: int) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+    """token_embed_bwd with gWc / gWi summed in an order that depends only on the ids and the shape (no float atomics);
+    gpos_c / gpos_i are token_embed_bwd's bit for bit"""
+    _req(conds, "conds", torch.int64); _req(codes, "codes", torch.int64); _req(g, "g")
+    B, Tc = conds.shape
+    Ti = codes.shape[1]
+    C = g.shape[-1]
+    L = _lib.lib()
+    ws_bytes = L.b200vq_token_embed_bwd_deterministic_workspace_bytes(B, Tc, Ti, C, Vc, Vi)
+    ws = torch.empty(max(ws_bytes, 1), device=g.device, dtype=torch.uint8)
+    gWc = torch.empty(Vc, C, device=g.device, dtype=torch.float32)
+    gWi = torch.empty(Vi, C, device=g.device, dtype=torch.float32)
+    gpc = torch.empty(Tc, C, device=g.device, dtype=torch.float32)
+    gpi = torch.empty(Ti, C, device=g.device, dtype=torch.float32)
+    _lib.check(L.b200vq_token_embed_bwd_deterministic(_p(conds), _p(codes), _p(g), _p(gWc), _p(gpc), _p(gWi), _p(gpi), B, Tc, Ti, C,
+                                                      Vc, Vi, _p(ws), ws_bytes, _stream()), "token_embed_bwd_deterministic")
     return gWc, gpc, gWi, gpi
 
 

@@ -61,7 +61,8 @@ class TokenEmbedFn(torch.autograd.Function):
     def backward(ctx, g):
         conds, codes = ctx.saved_tensors
         Vc, Vi, shape_c, shape_i = ctx.vocab
-        gWc, gpc, gWi, gpi = ops.token_embed_bwd(conds, codes, g.contiguous(), Vc, Vi)
+        bwd = ops.token_embed_bwd_deterministic if Fn.deterministic() else ops.token_embed_bwd
+        gWc, gpc, gWi, gpi = bwd(conds, codes, g.contiguous(), Vc, Vi)
         return None, None, gWc, gpc.view(shape_c), gWi, gpi.view(shape_i)
 
 

@@ -136,6 +136,15 @@ int b200vq_vq_fwd(const float* z, const float* E, float* out, long long* idx, fl
 int b200vq_vq_bwd(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss,
                   float* gz, float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm,
                   void* stream);
+/* bit-reproducible variant of b200vq_vq_bwd: the same gz (same arithmetic, bit for bit) and a gE whose summation order
+ * depends only on idx and the shape -- not on the SM count, b200vq_set_sm_limit or timing.  Each entry m*depth + t of
+ * idx (m for the plain quantiser) stores its codebook contribution in the workspace; a stable radix sort of the
+ * entries by code and a segmented sum in ascending entry order (fixed runs of entries, then the runs in order) make gE.
+ * No float atomics.  Same constraints as b200vq_vq_bwd plus n_embed % 4 == 0; workspace from the query below. */
+size_t b200vq_vq_bwd_deterministic_workspace_bytes(int M, int K, int D, int depth);
+int b200vq_vq_bwd_deterministic(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss,
+                                float* gz, float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm,
+                                void* workspace, size_t ws_bytes, void* stream);
 /* decode_codes (vitvqgan.py:81-86): out[m] = sum_t norm(E[codes[m,t]]) */
 int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
                     void* stream);
@@ -194,6 +203,9 @@ int b200vq_upfirdn2d(const float* in, const float* kernel, float* out, long long
  * sqrelu: grad 0: y = relu(x)^2 (layers.py:108); grad 1: y = g * 2 relu(x), x the pre-activation.
  * token_embed: x[b] = cat(Wc[conds[b]] + pos_c, Wi[codes[b]] + pos_i) (layers.py:199-206); conds int64 [B, Tc], codes
  *   int64 [B, Ti], x [B, Tc + Ti, C].  bwd: gWc / gWi are zero-filled then accumulated, gpos_* = sum over the batch.
+ *   bwd_deterministic: the same results with gWc / gWi summed in a fixed order (ids clamped as in bwd; the stable sort
+ *   and segmented sum of b200vq_vq_bwd_deterministic, no float atomics), gpos_* bit-identical to bwd's; Vc, Vi > 0;
+ *   workspace from its query.
  * copy_rows: dst[b, t] = src[b, t - off_dst + off_src] for off_dst <= t < off_dst + n, else 0 (the window
  *   x[:, cond-1:-1] of layers.py:210 and its zero-padded gradient).
  * decode_attention: one sampling step of layers.py:66-81 (use_cache with layer_past): appends the k / v thirds of
@@ -213,6 +225,10 @@ int b200vq_token_embed_fwd(const long long* conds, const long long* codes, const
                            const float* pos_i, float* x, int B, int Tc, int Ti, int C, int Vc, int Vi, void* stream);
 int b200vq_token_embed_bwd(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c, float* gWi,
                            float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* stream);
+size_t b200vq_token_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int Ti, int C, int Vc, int Vi);
+int b200vq_token_embed_bwd_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                         float* gWi, float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* workspace,
+                                         size_t ws_bytes, void* stream);
 int b200vq_copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, int off_src, int off_dst, int n, int C,
                      void* stream);
 int b200vq_decode_attention(const float* qkv, float* cache_k, float* cache_v, float* out, int B, int heads, int hs, int Tmax,
