@@ -34,6 +34,7 @@
 #include "common.cuh"
 
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 
 namespace b200 {
@@ -96,6 +97,9 @@ __device__ __forceinline__ uint32_t tile_off(int mn, int k) {
     return (uint32_t)(mn / El::ATOM) * (El::BK * 128u) + (uint32_t)k * 128u + ((((b >> 4) ^ (uint32_t)k) & 7u) << 4) + (b & 15u);
   }
 }
+
+__device__ __forceinline__ float2 pair_to_float2(float2 v) { return v; }
+__device__ __forceinline__ float2 pair_to_float2(uint32_t v) { return __half22float2(*reinterpret_cast<const __half2*>(&v)); }
 
 // P3: the 3xTF32 product (KIND 0, passes == 3), with per-k-block promotion of the partial sums
 template <int KIND, int BN, int AMAJ, int BMAJ, int OUT16, int P3>
@@ -275,64 +279,175 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
 
     if constexpr (WG) {
+      // ---------------------------------------------------------------- epilogue (rows g, g + 8 of each m16 tile)
+      // As far as the compiler knows the output may alias an epilogue input, so it keeps every load below the stores
+      // that precede it in the source: loading each n8 tile's inputs right before its stores would cost every warp one
+      // memory round trip per n8 tile.  The bias pairs and epilogue-input pairs are therefore loaded ahead of the stores,
+      // the first tile's before the last k-block's MMAs are waited for.  The lookahead grows only as fast as the stored
+      // tiles free their accumulator registers, up to kAheadMax tiles: ptxas caps the kernel at 168 registers (9 warps at
+      // one CTA per SM put 3 warps on one SM sub-partition's 16 K registers), and the fp16 kind's accumulators take 128.
+      // The loads are predicated rather than branched over: branches around them cost the allocator spills.  Every element
+      // goes through the same operations in the same order as when loaded in place, and is only ever loaded by the thread
+      // that stores it, before it stores it, so an output written in place over its epilogue input stays correct.
+      //
+      // One input slot per element pair ("ex"): the in_mode 1 / 2 input (output dtype), or else the residual-table row.
+      // With both (in_mode 2 and a table, fp32 output only) the table row is loaded where it is added.
+      using OutT = std::conditional_t<OUT16 != 0, __half, float>;
+      using ExPair = std::conditional_t<OUT16 != 0, uint32_t, float2>;   // an fp16 pair travels as its bits
+      constexpr int kTileRegs = 2 + MT * 2 * (OUT16 ? 1 : 2);          // one n8 tile's bias and input pairs
+      constexpr int kAheadMax = 8;
+      const int col0 = nb * BN + 2 * tq;                                // this thread's first column; n8 tile nt adds 8 nt
+      const bool has_bias = p.bias != nullptr, ex_is_in = p.in_mode != 0, has_ex = ex_is_in || p.res != nullptr;
+      bool row_ok[MT][2];
+      OutT* c_row[MT][2];
+      const ExPair* ex_row[MT][2];
+  #pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+  #pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = mb * kBM + warp * 16 + g + h * 8;
+          row_ok[mt][h] = row < p.M;
+          c_row[mt][h] = static_cast<OutT*>(p.C) + (long long)z * p.c_split_stride + (long long)row * p.ldc + col0;
+          ex_row[mt][h] = ex_is_in ? reinterpret_cast<const ExPair*>(static_cast<const OutT*>(p.in) + (long long)row * p.ldin + col0)
+                                   : reinterpret_cast<const ExPair*>(p.res + (long long)(row % (p.res_row_mod > 0 ? p.res_row_mod : 1)) * p.ldres + col0);
+        }
+      float2 bias_v[NTW];
+      ExPair ex_v[NTW][MT][2];
+      // N is even, so col < N implies col + 1 < N
+      auto fetch = [&](int nt) {
+        const bool col_ok = col0 + nt * 8 < p.N;
+        bias_v[nt] = has_bias && col_ok ? reinterpret_cast<const float2*>(p.bias + col0)[nt * 4] : make_float2(0.f, 0.f);
+  #pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) ex_v[nt][mt][h] = has_ex && row_ok[mt][h] && col_ok ? ex_row[mt][h][nt * 4] : ExPair{};
+      };
+      // tiles [0, fetched(nt)) are loaded before tile nt is stored: as many tiles ahead as the accumulator registers of
+      // the tiles already stored can hold, at least one and at most kAheadMax.
+      auto fetched = [](int nt) {
+        int ahead = 4 * MT * nt / kTileRegs;
+        ahead = ahead < 1 ? 1 : ahead > kAheadMax ? kAheadMax : ahead;
+        return nt + ahead < NTW ? nt + ahead : NTW;
+      };
+  #pragma unroll
+      for (int nt = 0; nt < fetched(0); ++nt) fetch(nt);
+
       wgmma_wait<0>();
       wgmma_fence_regs(d);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[held]);
-    }
 
-    // ---------------------------------------------------------------- epilogue (rows g, g + 8 of each m16 tile)
-    const long long zoff = (long long)z * p.c_split_stride;
-#pragma unroll
-    for (int nt = 0; nt < NTW; ++nt) {
-      const int col = nb * BN + (WG ? 0 : wn * WN) + nt * 8 + 2 * tq;
-      const bool col_ok = col < p.N;     // N is even, so col + 1 < N as well
-      float2 bias2 = make_float2(0.f, 0.f);
-      if (p.bias && col_ok) bias2 = *reinterpret_cast<const float2*>(p.bias + col);
-#pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
-        const int row16 = mb * kBM + (WG ? warp * 16 : wm * 32 + mt * 16);
-        float cs0 = 0.f, cs1 = 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {    // row half: g, g + 8
-          const int row = row16 + g + h * 8;
-          float o0 = acc[mt][nt][h * 2] * alpha + bias2.x;
-          float o1 = acc[mt][nt][h * 2 + 1] * alpha + bias2.y;
-          if (row >= p.M || !col_ok) continue;
-          if (p.act == 1) { o0 = fast_tanh(o0); o1 = fast_tanh(o1); }
-          if (p.in_mode == 1) {
-            const float2 a = *reinterpret_cast<const float2*>(static_cast<const float*>(p.in) + (long long)row * p.ldin + col);
-            o0 += a.x; o1 += a.y;
-          } else if (p.in_mode == 2) {
-            float2 a;
-            if constexpr (OUT16) a = __half22float2(*reinterpret_cast<const __half2*>(static_cast<const __half*>(p.in) + (long long)row * p.ldin + col));
-            else                 a = *reinterpret_cast<const float2*>(static_cast<const float*>(p.in) + (long long)row * p.ldin + col);
-            o0 *= 1.f - a.x * a.x; o1 *= 1.f - a.y * a.y;
+  #pragma unroll
+      for (int nt = 0; nt < NTW; ++nt) {
+  #pragma unroll
+        for (int f = nt == 0 ? fetched(0) : fetched(nt - 1); f < fetched(nt); ++f) fetch(f);
+        const int col = col0 + nt * 8;
+        const bool col_ok = col < p.N;
+        const float2 bias2 = bias_v[nt];
+  #pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          const int row16 = mb * kBM + (WG ? warp * 16 : wm * 32 + mt * 16);
+          float cs0 = 0.f, cs1 = 0.f;
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {    // row half: g, g + 8
+            float o0 = acc[mt][nt][h * 2] * alpha + bias2.x;
+            float o1 = acc[mt][nt][h * 2 + 1] * alpha + bias2.y;
+            if (!row_ok[mt][h] || !col_ok) continue;
+            if (p.act == 1) { o0 = fast_tanh(o0); o1 = fast_tanh(o1); }
+            const float2 a = pair_to_float2(ex_v[nt][mt][h]);
+            if constexpr (!OUT16) {          // fp16 output takes no fp32 residual (gemm_launch)
+              if (p.in_mode == 1) { o0 += a.x; o1 += a.y; }
+            }
+            if (p.in_mode == 2) { o0 *= 1.f - a.x * a.x; o1 *= 1.f - a.y * a.y; }
+            if constexpr (!OUT16) {
+              if (p.res) {
+                const int row = row16 + g + h * 8;
+                const float2 rr = ex_is_in ? *reinterpret_cast<const float2*>(p.res + (long long)(row % p.res_row_mod) * p.ldres + col) : a;
+                o0 += rr.x; o1 += rr.y;
+              }
+            }
+            if constexpr (OUT16) {
+              const uint32_t pk = pack_half2_sat(o0, o1);
+              reinterpret_cast<uint32_t*>(c_row[mt][h])[nt * 4] = pk;
+              const float2 st = __half22float2(*reinterpret_cast<const __half2*>(&pk));
+              cs0 += st.x; cs1 += st.y;
+            } else {
+              if (p.round_out) { o0 = round_tf32(o0); o1 = round_tf32(o1); }
+              reinterpret_cast<float2*>(c_row[mt][h])[nt * 4] = make_float2(o0, o1);
+              cs0 += o0; cs1 += o1;
+            }
           }
-          if (p.res) {
-            const float2 rr = *reinterpret_cast<const float2*>(p.res + (long long)(row % p.res_row_mod) * p.ldres + col);
-            o0 += rr.x; o1 += rr.y;
-          }
-          if constexpr (OUT16) {
-            const uint32_t pk = pack_half2_sat(o0, o1);
-            *reinterpret_cast<uint32_t*>(static_cast<__half*>(p.C) + zoff + (long long)row * p.ldc + col) = pk;
-            const float2 st = __half22float2(*reinterpret_cast<const __half2*>(&pk));
-            cs0 += st.x; cs1 += st.y;
-          } else {
-            if (p.round_out) { o0 = round_tf32(o0); o1 = round_tf32(o1); }
-            *reinterpret_cast<float2*>(static_cast<float*>(p.C) + zoff + (long long)row * p.ldc + col) = make_float2(o0, o1);
-            cs0 += o0; cs1 += o1;
+          if (p.colsum_part) {
+            // bias gradient for free: the m16 tile's rows are one 16-row group of the partial-sum table
+  #pragma unroll
+            for (int off = 4; off < 32; off <<= 1) {
+              cs0 += __shfl_xor_sync(0xffffffffu, cs0, off);
+              cs1 += __shfl_xor_sync(0xffffffffu, cs1, off);
+            }
+            if (g == 0 && col_ok && row16 < p.M)
+              *reinterpret_cast<float2*>(p.colsum_part + (size_t)(row16 >> 4) * p.N + col) = make_float2(cs0, cs1);
           }
         }
-        if (p.colsum_part) {
-          // bias gradient for free: the m16 tile's rows are one 16-row group of the partial-sum table
-#pragma unroll
-          for (int off = 4; off < 32; off <<= 1) {
-            cs0 += __shfl_xor_sync(0xffffffffu, cs0, off);
-            cs1 += __shfl_xor_sync(0xffffffffu, cs1, off);
+      }
+    } else {
+      // tf32 kinds: each element pair's inputs are loaded where they are used.  The same loads run ahead of the
+      // stores, as above, changed results from launch to launch once a CTA ran several tiles with column sums
+      // (test_gemm_epilogue_input_refill_is_race_free): whole n8 tiles of a warp came out wrong, which points at the
+      // mma.sync main loop's shared-memory fragment loads and the stage release under a different schedule, not at
+      // the epilogue.  Not resolved; these kinds keep the schedule they were validated with.
+      // ---------------------------------------------------------------- epilogue (rows g, g + 8 of each m16 tile)
+      const long long zoff = (long long)z * p.c_split_stride;
+  #pragma unroll
+      for (int nt = 0; nt < NTW; ++nt) {
+        const int col = nb * BN + (WG ? 0 : wn * WN) + nt * 8 + 2 * tq;
+        const bool col_ok = col < p.N;     // N is even, so col + 1 < N as well
+        float2 bias2 = make_float2(0.f, 0.f);
+        if (p.bias && col_ok) bias2 = *reinterpret_cast<const float2*>(p.bias + col);
+  #pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          const int row16 = mb * kBM + (WG ? warp * 16 : wm * 32 + mt * 16);
+          float cs0 = 0.f, cs1 = 0.f;
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {    // row half: g, g + 8
+            const int row = row16 + g + h * 8;
+            float o0 = acc[mt][nt][h * 2] * alpha + bias2.x;
+            float o1 = acc[mt][nt][h * 2 + 1] * alpha + bias2.y;
+            if (row >= p.M || !col_ok) continue;
+            if (p.act == 1) { o0 = fast_tanh(o0); o1 = fast_tanh(o1); }
+            if (p.in_mode == 1) {
+              const float2 a = *reinterpret_cast<const float2*>(static_cast<const float*>(p.in) + (long long)row * p.ldin + col);
+              o0 += a.x; o1 += a.y;
+            } else if (p.in_mode == 2) {
+              float2 a;
+              if constexpr (OUT16) a = __half22float2(*reinterpret_cast<const __half2*>(static_cast<const __half*>(p.in) + (long long)row * p.ldin + col));
+              else                 a = *reinterpret_cast<const float2*>(static_cast<const float*>(p.in) + (long long)row * p.ldin + col);
+              o0 *= 1.f - a.x * a.x; o1 *= 1.f - a.y * a.y;
+            }
+            if (p.res) {
+              const float2 rr = *reinterpret_cast<const float2*>(p.res + (long long)(row % p.res_row_mod) * p.ldres + col);
+              o0 += rr.x; o1 += rr.y;
+            }
+            if constexpr (OUT16) {
+              const uint32_t pk = pack_half2_sat(o0, o1);
+              *reinterpret_cast<uint32_t*>(static_cast<__half*>(p.C) + zoff + (long long)row * p.ldc + col) = pk;
+              const float2 st = __half22float2(*reinterpret_cast<const __half2*>(&pk));
+              cs0 += st.x; cs1 += st.y;
+            } else {
+              if (p.round_out) { o0 = round_tf32(o0); o1 = round_tf32(o1); }
+              *reinterpret_cast<float2*>(static_cast<float*>(p.C) + zoff + (long long)row * p.ldc + col) = make_float2(o0, o1);
+              cs0 += o0; cs1 += o1;
+            }
           }
-          if (g == 0 && col_ok && row16 < p.M)
-            *reinterpret_cast<float2*>(p.colsum_part + (size_t)(row16 >> 4) * p.N + col) = make_float2(cs0, cs1);
+          if (p.colsum_part) {
+            // bias gradient for free: the m16 tile's rows are one 16-row group of the partial-sum table
+  #pragma unroll
+            for (int off = 4; off < 32; off <<= 1) {
+              cs0 += __shfl_xor_sync(0xffffffffu, cs0, off);
+              cs1 += __shfl_xor_sync(0xffffffffu, cs1, off);
+            }
+            if (g == 0 && col_ok && row16 < p.M)
+              *reinterpret_cast<float2*>(p.colsum_part + (size_t)(row16 >> 4) * p.N + col) = make_float2(cs0, cs1);
+          }
         }
       }
     }
