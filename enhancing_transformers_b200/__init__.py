@@ -14,11 +14,11 @@ from .layers import (Attention, FeedForward, PosQuantLinear, PreNorm, QuantLinea
 from .parallel import FlatGradients, allreduce_gradients  # noqa: F401
 from .quantizers import BaseQuantizer, GumbelQuantizer, VectorQuantizer  # noqa: F401
 from . import stage2  # noqa: F401
-from .stage2 import GPT  # noqa: F401
+from .stage2 import GPT, RQTransformer  # noqa: F401
 
 __version__ = "0.2.0"
 __all__ = ["ViTEncoder", "ViTDecoder", "VectorQuantizer", "GumbelQuantizer", "BaseQuantizer", "Transformer", "Attention", "FeedForward",
-           "PreNorm", "QuantLinear", "PosQuantLinear", "fuse_post_quant_pos", "detach_discriminator_forward", "GPT", "stage2", "patch", "patch_stage2", "install_as_reference_modules", "fuse_quant_linears", "set_precision",
+           "PreNorm", "QuantLinear", "PosQuantLinear", "fuse_post_quant_pos", "detach_discriminator_forward", "GPT", "RQTransformer", "stage2", "patch", "patch_stage2", "install_as_reference_modules", "fuse_quant_linears", "set_precision",
            "get_precision", "invalidate_shadows", "allreduce_gradients", "FlatGradients", "ops", "functional", "configs"]
 
 _REF_PKG = "enhancing.modules.stage1"
@@ -40,14 +40,14 @@ def patch(vitvqgan_module=None):
 
 
 def patch_stage2(layers_module=None):
-    """Rebind ``GPT`` (and its building blocks) inside the reference's ``enhancing.modules.stage2.layers``: the YAML's
+    """Rebind ``GPT``, ``RQTransformer`` (and their building blocks) inside the reference's ``enhancing.modules.stage2.layers``: the YAML's
     ``transformer.target: enhancing.modules.stage2.layers.GPT`` (configs/imagenet_gpt_vitvq_base.yaml:32-33) is resolved by
     attribute lookup on that module when ``CondTransformer.__init__`` runs (stage2/transformer.py:41), so the unchanged
     LightningModule constructs this package's classes.  The reference file itself is not edited."""
     if layers_module is None:
         import importlib
         layers_module = importlib.import_module("enhancing.modules.stage2.layers")
-    for name in ("GPT", "Block", "FFN", "MultiHeadSelfAttention"):
+    for name in ("GPT", "RQTransformer", "Block", "FFN", "MultiHeadSelfAttention"):
         setattr(layers_module, name, getattr(stage2, name))
     return layers_module
 

@@ -65,6 +65,17 @@ _SIGNATURES = {
     "b200vq_token_embed_bwd_deterministic": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_f, c_sz, c_f]),
     "b200vq_copy_rows": (c_i, [c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_decode_attention": (c_i, [c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_fl, c_f]),
+    "b200vq_short_attention_fwd": (c_i, [c_f, c_f, c_ll, c_i, c_i, c_i, c_i, c_fl, c_f]),
+    "b200vq_short_attention_bwd": (c_i, [c_f, c_f, c_f, c_ll, c_i, c_i, c_i, c_i, c_fl, c_f]),
+    "b200vq_rq_embed_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
+    "b200vq_rq_embed_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
+    "b200vq_rq_embed_bwd_deterministic_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i, c_i, c_i, c_i]),
+    "b200vq_rq_embed_bwd_deterministic": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f, c_sz, c_f]),
+    "b200vq_rq_depth_input_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_ll, c_i, c_i, c_i, c_f]),
+    "b200vq_rq_depth_input_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_ll, c_i, c_i, c_i, c_f]),
+    "b200vq_rq_depth_input_bwd_deterministic_workspace_bytes": (c_sz, [c_ll, c_i, c_i, c_i]),
+    "b200vq_rq_depth_input_bwd_deterministic": (c_i, [c_f, c_f, c_f, c_f, c_f, c_ll, c_i, c_i, c_i, c_f, c_sz, c_f]),
+    "b200vq_code_sum_embed": (c_i, [c_f, c_ll, c_i, c_f, c_f, c_f, c_i, c_i, c_i, c_f]),
 }
 EXPORTS = tuple(_SIGNATURES)
 

@@ -112,6 +112,21 @@ int token_embed_backward_deterministic(const long long*, const long long*, const
                                        int, int, int, void*, size_t, cudaStream_t);
 int copy_rows(const float*, float*, int, int, int, int, int, int, int, cudaStream_t);
 int decode_attention(const float*, float*, float*, float*, int, int, int, int, int, float, cudaStream_t);
+int short_attention_forward(const float*, float*, long long, int, int, int, int, float, cudaStream_t);
+int short_attention_backward(const float*, const float*, float*, long long, int, int, int, int, float, cudaStream_t);
+int rq_embed_forward(const long long*, const long long*, const float*, const float*, const float*, const float*, float*, int, int, int,
+                     int, int, int, int, cudaStream_t);
+int rq_embed_backward(const long long*, const long long*, const float*, float*, float*, float*, float*, int, int, int, int, int, int,
+                      int, cudaStream_t);
+size_t rq_embed_bwd_deterministic_workspace_bytes(int, int, int, int, int, int, int);
+int rq_embed_backward_deterministic(const long long*, const long long*, const float*, float*, float*, float*, float*, int, int, int, int,
+                                    int, int, int, void*, size_t, cudaStream_t);
+int rq_depth_input_forward(const float*, const long long*, const float*, const float*, float*, long long, int, int, int, cudaStream_t);
+int rq_depth_input_backward(const long long*, const float*, float*, float*, float*, long long, int, int, int, cudaStream_t);
+size_t rq_depth_input_bwd_deterministic_workspace_bytes(long long, int, int, int);
+int rq_depth_input_backward_deterministic(const long long*, const float*, float*, float*, float*, long long, int, int, int, void*, size_t,
+                                          cudaStream_t);
+int code_sum_embed(const long long*, long long, int, const float*, const float*, float*, int, int, int, cudaStream_t);
 
 }  // namespace b200
 
@@ -290,6 +305,51 @@ int b200vq_copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, 
 int b200vq_decode_attention(const float* qkv, float* cache_k, float* cache_v, float* out, int B, int heads, int hs, int Tmax,
                             int pos, float scale, void* stream) {
   return decode_attention(qkv, cache_k, cache_v, out, B, heads, hs, Tmax, pos, scale, S(stream));
+}
+
+int b200vq_short_attention_fwd(const float* qkv, float* out, long long nseq, int D, int heads, int hs, int cond_len, float scale,
+                               void* stream) {
+  return short_attention_forward(qkv, out, nseq, D, heads, hs, cond_len, scale, S(stream));
+}
+int b200vq_short_attention_bwd(const float* qkv, const float* dout, float* dqkv, long long nseq, int D, int heads, int hs, int cond_len,
+                               float scale, void* stream) {
+  return short_attention_backward(qkv, dout, dqkv, nseq, D, heads, hs, cond_len, scale, S(stream));
+}
+int b200vq_rq_embed_fwd(const long long* conds, const long long* codes, const float* Wc, const float* pos_c, const float* Wi,
+                        const float* pos_i, float* x, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* stream) {
+  return rq_embed_forward(conds, codes, Wc, pos_c, Wi, pos_i, x, B, Tc, T, D, C, Vc, Vi, S(stream));
+}
+int b200vq_rq_embed_bwd(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c, float* gWi,
+                        float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* stream) {
+  return rq_embed_backward(conds, codes, g, gWc, gpos_c, gWi, gpos_i, B, Tc, T, D, C, Vc, Vi, S(stream));
+}
+size_t b200vq_rq_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int T, int D, int C, int Vc, int Vi) {
+  return rq_embed_bwd_deterministic_workspace_bytes(B, Tc, T, D, C, Vc, Vi);
+}
+int b200vq_rq_embed_bwd_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                      float* gWi, float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* workspace,
+                                      size_t ws_bytes, void* stream) {
+  return rq_embed_backward_deterministic(conds, codes, g, gWc, gpos_c, gWi, gpos_i, B, Tc, T, D, C, Vc, Vi, workspace, ws_bytes,
+                                         S(stream));
+}
+int b200vq_rq_depth_input_fwd(const float* h, const long long* codes, const float* Wi, const float* pos_d, float* v, long long nseq,
+                              int D, int C, int Vi, void* stream) {
+  return rq_depth_input_forward(h, codes, Wi, pos_d, v, nseq, D, C, Vi, S(stream));
+}
+int b200vq_rq_depth_input_bwd(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq, int D, int C,
+                              int Vi, void* stream) {
+  return rq_depth_input_backward(codes, g, gh, gWi, gpos_d, nseq, D, C, Vi, S(stream));
+}
+size_t b200vq_rq_depth_input_bwd_deterministic_workspace_bytes(long long nseq, int D, int C, int Vi) {
+  return rq_depth_input_bwd_deterministic_workspace_bytes(nseq, D, C, Vi);
+}
+int b200vq_rq_depth_input_bwd_deterministic(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq,
+                                            int D, int C, int Vi, void* workspace, size_t ws_bytes, void* stream) {
+  return rq_depth_input_backward_deterministic(codes, g, gh, gWi, gpos_d, nseq, D, C, Vi, workspace, ws_bytes, S(stream));
+}
+int b200vq_code_sum_embed(const long long* codes, long long ld, int n, const float* Wi, const float* pos, float* out, int B, int C, int Vi,
+                          void* stream) {
+  return code_sum_embed(codes, ld, n, Wi, pos, out, B, C, Vi, S(stream));
 }
 
 }  // extern "C"

@@ -506,3 +506,105 @@ def decode_attention(qkv: Tensor, cache_k: Tensor, cache_v: Tensor, heads: int, 
     _lib.check(_lib.lib().b200vq_decode_attention(_p(qkv), _p(cache_k), _p(cache_v), _p(out), B, heads, hs, cache_k.shape[1], int(pos),
                                                   scale, _stream()), "decode_attention")
     return out
+
+
+# ----------------------------------------------------------------- stage-2 RQTransformer (reference layers.py:306-547)
+def short_attention_fwd(qkv: Tensor, nseq: int, D: int, heads: int, hs: int, scale: float, cond_len: int = 0) -> Tensor:
+    """causal attention over nseq independent sequences of D <= 16 tokens: qkv [nseq*D, 3C] -> out [nseq*D, C] (fp32 FMA)"""
+    _req(qkv, "qkv")
+    out = torch.empty(nseq * D, heads * hs, device=qkv.device, dtype=torch.float32)
+    _lib.check(_lib.lib().b200vq_short_attention_fwd(_p(qkv), _p(out), nseq, D, heads, hs, int(cond_len), scale, _stream()),
+               "short_attention_fwd")
+    return out
+
+
+def short_attention_bwd(qkv: Tensor, dout: Tensor, nseq: int, D: int, heads: int, hs: int, scale: float, cond_len: int = 0) -> Tensor:
+    """dqkv [nseq*D, 3C], the scores recomputed from qkv"""
+    _req(qkv, "qkv"); _req(dout, "dout")
+    dqkv = torch.empty_like(qkv)
+    _lib.check(_lib.lib().b200vq_short_attention_bwd(_p(qkv), _p(dout), _p(dqkv), nseq, D, heads, hs, int(cond_len), scale, _stream()),
+               "short_attention_bwd")
+    return dqkv
+
+
+def rq_embed_fwd(conds: Tensor, codes: Tensor, Wc: Tensor, pos_c: Tensor, Wi: Tensor, pos_i: Tensor) -> Tensor:
+    """conds int64 [B, Tc], codes int64 [B, T, D] -> x [B * (Tc + T), C]: cond rows Wc[conds] + pos_c, code rows
+    cumsum_C(Wi[codes[..., D-1]]) + pos_i"""
+    _req(conds, "conds", torch.int64); _req(codes, "codes", torch.int64)
+    _req(Wc, "tok_emb_cond.weight"); _req(pos_c, "pos_emb_cond"); _req(Wi, "tok_emb_code.weight"); _req(pos_i, "pos_emb_code")
+    B, Tc = conds.shape
+    _, T, D = codes.shape
+    C = Wi.shape[1]
+    x = torch.empty(B * (Tc + T), C, device=Wi.device, dtype=torch.float32)
+    _lib.check(_lib.lib().b200vq_rq_embed_fwd(_p(conds), _p(codes), _p(Wc), _p(pos_c), _p(Wi), _p(pos_i), _p(x), B, Tc, T, D, C,
+                                              Wc.shape[0], Wi.shape[0], _stream()), "rq_embed_fwd")
+    return x
+
+
+def rq_embed_bwd(conds: Tensor, codes: Tensor, g: Tensor, Vc: int, Vi: int,
+                 deterministic: bool = False) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+    """-> (gWc [Vc, C], gpos_c [Tc, C], gWi [Vi, C], gpos_i [T, C]); deterministic: gWc / gWi summed in a fixed order"""
+    _req(conds, "conds", torch.int64); _req(codes, "codes", torch.int64); _req(g, "g")
+    B, Tc = conds.shape
+    _, T, D = codes.shape
+    C = g.shape[-1]
+    gWc = torch.empty(Vc, C, device=g.device, dtype=torch.float32)
+    gWi = torch.empty(Vi, C, device=g.device, dtype=torch.float32)
+    gpc = torch.empty(Tc, C, device=g.device, dtype=torch.float32)
+    gpi = torch.empty(T, C, device=g.device, dtype=torch.float32)
+    L = _lib.lib()
+    args = (_p(conds), _p(codes), _p(g), _p(gWc), _p(gpc), _p(gWi), _p(gpi), B, Tc, T, D, C, Vc, Vi)
+    if deterministic:
+        ws_bytes = L.b200vq_rq_embed_bwd_deterministic_workspace_bytes(B, Tc, T, D, C, Vc, Vi)
+        ws = torch.empty(max(ws_bytes, 1), device=g.device, dtype=torch.uint8)
+        _lib.check(L.b200vq_rq_embed_bwd_deterministic(*args, _p(ws), ws_bytes, _stream()), "rq_embed_bwd_deterministic")
+    else:
+        _lib.check(L.b200vq_rq_embed_bwd(*args, _stream()), "rq_embed_bwd")
+    return gWc, gpc, gWi, gpi
+
+
+def rq_depth_input_fwd(h: Tensor, codes: Tensor, Wi: Tensor, pos_d: Tensor) -> Tensor:
+    """h [B*T, C], codes int64 [B, T, D], pos_d [D-1, C] -> v [B*T*D, C]: v[s, 0] = h[s], v[s, d] = cumsum_C(Wi[codes[s, d-1]]) +
+    pos_d[d-1]"""
+    _req(h, "h"); _req(codes, "codes", torch.int64); _req(Wi, "tok_emb_code.weight"); _req(pos_d, "pos_emb_depth")
+    D = codes.shape[-1]
+    nseq = codes.numel() // D
+    C = Wi.shape[1]
+    v = torch.empty(nseq * D, C, device=h.device, dtype=torch.float32)
+    _lib.check(_lib.lib().b200vq_rq_depth_input_fwd(_p(h), _p(codes), _p(Wi), _p(pos_d), _p(v), nseq, D, C, Wi.shape[0], _stream()),
+               "rq_depth_input_fwd")
+    return v
+
+
+def rq_depth_input_bwd(codes: Tensor, g: Tensor, Vi: int, deterministic: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
+    """-> (gh [B*T, C], gWi [Vi, C], gpos_d [D-1, C]); deterministic: gWi summed in a fixed order"""
+    _req(codes, "codes", torch.int64); _req(g, "g")
+    D = codes.shape[-1]
+    nseq = codes.numel() // D
+    C = g.shape[-1]
+    gh = torch.empty(nseq, C, device=g.device, dtype=torch.float32)
+    gWi = torch.empty(Vi, C, device=g.device, dtype=torch.float32)
+    gpd = torch.empty(D - 1, C, device=g.device, dtype=torch.float32)
+    L = _lib.lib()
+    args = (_p(codes), _p(g), _p(gh), _p(gWi), _p(gpd), nseq, D, C, Vi)
+    if deterministic:
+        ws_bytes = L.b200vq_rq_depth_input_bwd_deterministic_workspace_bytes(nseq, D, C, Vi)
+        ws = torch.empty(max(ws_bytes, 1), device=g.device, dtype=torch.uint8)
+        _lib.check(L.b200vq_rq_depth_input_bwd_deterministic(*args, _p(ws), ws_bytes, _stream()), "rq_depth_input_bwd_deterministic")
+    else:
+        _lib.check(L.b200vq_rq_depth_input_bwd(*args, _stream()), "rq_depth_input_bwd")
+    return gh, gWi, gpd
+
+
+def code_sum_embed(codes: Tensor, n: int, Wi: Tensor, pos: Tensor) -> Tensor:
+    """codes int64 [B, >= n] (rows may be strided; each row's first n entries are read) -> out [B, C] =
+    sum_{j < n} Wi[codes[b, j]] + pos (one [C] row)"""
+    _req(Wi, "tok_emb_code.weight"); _req(pos, "pos")
+    if not codes.is_cuda or codes.dtype != torch.int64 or codes.stride(1) != 1:
+        raise RuntimeError("b200vq: `codes` must be a CUDA int64 matrix with unit column stride")
+    B = codes.shape[0]
+    C = Wi.shape[1]
+    out = torch.empty(B, C, device=Wi.device, dtype=torch.float32)
+    _lib.check(_lib.lib().b200vq_code_sum_embed(_p(codes), codes.stride(0), int(n), _p(Wi), _p(pos), _p(out), B, C, Wi.shape[0], _stream()),
+               "code_sum_embed")
+    return out

@@ -15,6 +15,10 @@ tf32; "parity" -> 3xTF32 GEMMs and attention (fp32-grade).  Limits of the kernel
 head size ``embed_dim // n_heads`` must be 32 or 64, ``embed_dim`` <= 2048, ``vocab_img_size`` % 64 == 0 (the YAML's 6144 / 16 = 384-wide heads --
 a 10.9 B-parameter model that cannot train under replicated fp32 DDP anyway, SURVEY.md section 8f-3 -- are not covered).
 
+``RQTransformer`` (reference :306-547, the prior over residual codes [B, T, D]) reuses these blocks: its spatial transformer is
+``GPT``'s, its depth transformer runs causal attention over B*T sequences of D <= 16 tokens on the short-sequence kernel of
+csrc/rq_stage2.cu (fp32 FMA on every data path), and its channel-cumsum code embeddings are HBM streams there too.
+
 There is no CPU path: CPU tensors raise (use the reference classes on CPU)."""
 from __future__ import annotations
 
@@ -208,6 +212,63 @@ class RowWindowFn(torch.autograd.Function):
         return ops.copy_rows(g.contiguous(), B, n, T, 0, off, n), None, None, None, None
 
 
+class ShortAttentionFn(torch.autograd.Function):
+    """the masked attention core over nseq independent sequences of D <= 16 tokens (the depth transformer's blocks,
+    reference stage2/layers.py:346-352 with ctx_len = D, cond_len = 0): one warp per (sequence, head), fp32 FMA"""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, qkv, nseq, D, heads, hs, cond_len):
+        scale = 1.0 / math.sqrt(hs)
+        ctx.save_for_backward(qkv)
+        ctx.dims = (nseq, D, heads, hs, cond_len, scale)
+        return ops.short_attention_fwd(qkv, nseq, D, heads, hs, scale, cond_len)
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        (qkv,) = ctx.saved_tensors
+        nseq, D, heads, hs, cond_len, scale = ctx.dims
+        return ops.short_attention_bwd(qkv, g.contiguous(), nseq, D, heads, hs, scale, cond_len), None, None, None, None, None
+
+
+class RQEmbedFn(torch.autograd.Function):
+    """the spatial input of RQTransformer.forward (reference stage2/layers.py:374-384): cat(tok_emb_cond(conds) + pos_emb_cond,
+    tok_emb_code(codes).cumsum(-1)[..., -1, :] + pos_emb_code) -- the cumsum runs over the channels, so only the last depth's
+    code enters"""
+
+    @staticmethod
+    def forward(ctx, conds, codes, Wc, pos_c, Wi, pos_i):
+        ctx.save_for_backward(conds, codes)
+        ctx.vocab = (Wc.shape[0], Wi.shape[0], pos_c.shape, pos_i.shape)
+        return ops.rq_embed_fwd(conds, codes, Wc, pos_c, Wi, pos_i)
+
+    @staticmethod
+    def backward(ctx, g):
+        conds, codes = ctx.saved_tensors
+        Vc, Vi, shape_c, shape_i = ctx.vocab
+        gWc, gpc, gWi, gpi = ops.rq_embed_bwd(conds, codes, g.contiguous(), Vc, Vi, deterministic=Fn.deterministic())
+        return None, None, gWc, gpc.view(shape_c), gWi, gpi.view(shape_i)
+
+
+class RQDepthInputFn(torch.autograd.Function):
+    """the depth input of RQTransformer.forward (reference stage2/layers.py:388-391): per code position, row 0 is the spatial
+    hidden state h, row d >= 1 is tok_emb_code(codes[..., d-1]).cumsum(-1) + pos_emb_depth[d-1]"""
+
+    @staticmethod
+    def forward(ctx, h, codes, Wi, pos_d):
+        ctx.save_for_backward(codes)
+        ctx.meta = (Wi.shape[0], pos_d.shape)
+        return ops.rq_depth_input_fwd(h, codes, Wi, pos_d)
+
+    @staticmethod
+    def backward(ctx, g):
+        (codes,) = ctx.saved_tensors
+        Vi, shape_d = ctx.meta
+        gh, gWi, gpd = ops.rq_depth_input_bwd(codes, g.contiguous(), Vi, deterministic=Fn.deterministic())
+        return gh, None, gWi, gpd.view(shape_d)
+
+
 def _check_kernel_limits(embed_dim: int, n_heads: int) -> None:
     assert embed_dim % n_heads == 0
     hs = embed_dim // n_heads
@@ -229,6 +290,8 @@ class MultiHeadSelfAttention(nn.Module):
         self.value = nn.Linear(embed_dim, embed_dim, bias=attn_bias)
         self.proj = nn.Linear(embed_dim, embed_dim, attn_bias)
         self.n_heads, self.ctx_len, self.cond_len, self.use_mask = n_heads, ctx_len, cond_len, use_mask
+        # set by RQTransformer on its depth blocks: B*T sequences of ctx_len <= 16 tokens go to the short-sequence kernel
+        self.short_seq = False
         if use_mask:       # never read by the kernels (the mask is two integers there); kept for module-tree parity
             mask = torch.tril(torch.ones(ctx_len, ctx_len)).view(1, ctx_len, ctx_len)
             mask[:, :cond_len, :cond_len] = 1
@@ -250,7 +313,10 @@ class MultiHeadSelfAttention(nn.Module):
         w, b = self.packed_qkv()
         qkv = _linear(mixed, w, b)
         cond = min(self.cond_len, T) if self.use_mask else T      # no mask == every key visible == a prefix of T tokens
-        o = CausalAttentionFn.apply(qkv, B, T, self.n_heads, C // self.n_heads, cond)
+        if self.short_seq:
+            o = ShortAttentionFn.apply(qkv, B, T, self.n_heads, C // self.n_heads, cond)
+        else:
+            o = CausalAttentionFn.apply(qkv, B, T, self.n_heads, C // self.n_heads, cond)
         return _linear(o, self.proj.weight, self.proj.bias, res)
 
     def forward(self, x: Tensor, use_cache: bool = False, layer_past=None):
@@ -303,6 +369,67 @@ class Block(nn.Module):
 
     def sample(self, x, layer_past=None):
         raise NotImplementedError("b200vq stage 2: use GPT.sample / GPT.sample_step (the KV cache is owned by GPT)")
+
+
+def _cached_prefix(blocks, x: Tensor, B: int, T: int, ctx: int, heads: int, hs: int):
+    """the first sampling step of a block stack (reference stage2/layers.py:139-143 with layer_past None) over x [B*T, C]:
+    T tokens that see each other fully (the condition prefix, :83-85 with T == cond_len; or one token).  Allocates each
+    layer's key / value cache [B, ctx, C] and fills its first T rows.  -> (x, past)"""
+    C = x.shape[-1]
+    past = {"k": [], "v": [], "len": T}
+    for block in blocks:
+        att = block.attn
+        h = Fn.LayerNormFn.apply(x, block.ln1.weight, block.ln1.bias, False)
+        mixed = ops.time_mix_fwd(h, att.time_mix.view(-1), T)
+        w, b = att.packed_qkv()
+        qkv = _linear(mixed, w, b)
+        ck = torch.zeros(B, ctx, C, device=x.device)
+        cv = torch.zeros(B, ctx, C, device=x.device)
+        q3 = qkv.view(B, T, 3, C)
+        ck[:, :T] = q3[:, :, 1]
+        cv[:, :T] = q3[:, :, 2]
+        past["k"].append(ck)
+        past["v"].append(cv)
+        o = CausalAttentionFn.apply(qkv, B, T, heads, hs, T)
+        x = _linear(o, att.proj.weight, att.proj.bias, x)
+        x = block.mlp.core(Fn.LayerNormFn.apply(x, block.ln2.weight, block.ln2.bias, False), res=x)
+    return x, past
+
+
+def _cached_step(blocks, x: Tensor, past: dict, heads: int, hs: int) -> Tensor:
+    """one later sampling step of a block stack over x [B, C] (reference stage2/layers.py:139-143 with layer_past): the key /
+    value rows go to cache row past["len"], the query attends to rows 0 .. past["len"] unmasked (:76-81)"""
+    pos = past["len"]
+    scale = 1.0 / math.sqrt(hs)
+    for li, block in enumerate(blocks):
+        att = block.attn
+        h = Fn.LayerNormFn.apply(x, block.ln1.weight, block.ln1.bias, False)
+        mixed = ops.time_mix_fwd(h, att.time_mix.view(-1), 1)
+        w, b = att.packed_qkv()
+        qkv = _linear(mixed, w, b)
+        o = ops.decode_attention(qkv, past["k"][li], past["v"][li], heads, hs, pos, scale)
+        x = _linear(o, att.proj.weight, att.proj.bias, x)
+        x = block.mlp.core(Fn.LayerNormFn.apply(x, block.ln2.weight, block.ln2.bias, False), res=x)
+    past["len"] = pos + 1
+    return x
+
+
+def _filter_and_draw(logits_: Tensor, top_k, top_p) -> Tensor:
+    """the top-k / nucleus filtering and multinomial draw of the reference's samplers (stage2/layers.py:242-260, :448-466),
+    call for call, so that the same torch RNG stream draws the same codes"""
+    if top_k is not None:
+        v, ix = torch.topk(logits_, top_k)
+        logits_[logits_ < v[:, [-1]]] = -float('Inf')
+    probs = F.softmax(logits_, dim=-1)
+    if top_p is not None:
+        sorted_probs, sorted_indices = torch.sort(probs, dim=-1, descending=True)
+        cum_probs = torch.cumsum(sorted_probs, dim=-1)
+        remove = cum_probs >= top_p
+        remove[..., 1:] = remove[..., :-1].clone()
+        remove[..., 0] = 0
+        probs = probs.masked_fill(remove.scatter(-1, sorted_indices, remove), 0.0)
+        probs = probs / torch.sum(probs, dim=-1, keepdim=True)
+    return torch.multinomial(probs, num_samples=1).clone().detach()
 
 
 class GPT(nn.Module):
@@ -370,19 +497,7 @@ class GPT(nn.Module):
                 pos_code = self.pos_emb_code[:, i - 1:i, :]
             logits_, past = self.sample_step(codes_, conds, pos_code, use_fp16, past)
             logits_ = logits_.to(dtype=torch.float32) / softmax_temperature
-            if top_k is not None:
-                v, ix = torch.topk(logits_, top_k)
-                logits_[logits_ < v[:, [-1]]] = -float('Inf')
-            probs = F.softmax(logits_, dim=-1)
-            if top_p is not None:
-                sorted_probs, sorted_indices = torch.sort(probs, dim=-1, descending=True)
-                cum_probs = torch.cumsum(sorted_probs, dim=-1)
-                remove = cum_probs >= top_p
-                remove[..., 1:] = remove[..., :-1].clone()
-                remove[..., 0] = 0
-                probs = probs.masked_fill(remove.scatter(-1, sorted_indices, remove), 0.0)
-                probs = probs / torch.sum(probs, dim=-1, keepdim=True)
-            idx = torch.multinomial(probs, num_samples=1).clone().detach()
+            idx = _filter_and_draw(logits_, top_k, top_p)
             codes = idx if codes is None else torch.cat([codes, idx], axis=1)
             logits = logits_ if logits is None else torch.cat([logits, logits_], axis=1)
         del past
@@ -395,7 +510,6 @@ class GPT(nn.Module):
         C = self.head.weight.shape[1]
         heads = self.blocks[0].attn.n_heads if len(self.blocks) else 1
         hs = C // heads
-        scale = 1.0 / math.sqrt(hs)
         if codes is None:
             assert past is None
             conds = conds.contiguous()
@@ -405,43 +519,161 @@ class GPT(nn.Module):
             empty = torch.empty(B, 0, dtype=torch.int64, device=dev)
             x = ops.token_embed_fwd(conds, empty, self.tok_emb_cond.weight, self.pos_emb_cond.view(Tc, C),
                                     self.tok_emb_code.weight, self.pos_emb_code.view(-1, C))
-            past = {"k": [], "v": [], "len": Tc}
-            for block in self.blocks:
-                att = block.attn
-                h = Fn.LayerNormFn.apply(x, block.ln1.weight, block.ln1.bias, False)
-                mixed = ops.time_mix_fwd(h, att.time_mix.view(-1), Tc)
-                w, b = att.packed_qkv()
-                qkv = _linear(mixed, w, b)
-                ck = torch.zeros(B, ctx, C, device=dev)
-                cv = torch.zeros(B, ctx, C, device=dev)
-                q3 = qkv.view(B, Tc, 3, C)
-                ck[:, :Tc] = q3[:, :, 1]
-                cv[:, :Tc] = q3[:, :, 2]
-                past["k"].append(ck)
-                past["v"].append(cv)
-                o = CausalAttentionFn.apply(qkv, B, Tc, heads, hs, Tc)      # the condition prefix sees itself fully (:83-85 with T == cond_len)
-                x = _linear(o, att.proj.weight, att.proj.bias, x)
-                x = block.mlp.core(Fn.LayerNormFn.apply(x, block.ln2.weight, block.ln2.bias, False), res=x)
+            x, past = _cached_prefix(self.blocks, x, B, Tc, ctx, heads, hs)
             x = Fn.LayerNormFn.apply(x, self.layer_norm.weight, self.layer_norm.bias, False)
             x = ops.copy_rows(x, B, Tc, 1, Tc - 1, 0, 1)
         else:
             assert past is not None
             B = codes.shape[0]
-            pos = past["len"]
             # a one-token sequence: time_shift(x) is all zeros (reference :58 on T == 1), so the mix is x * time_mix + 0
             x = ops.token_embed_fwd(torch.empty(B, 0, dtype=torch.int64, device=codes.device), codes.contiguous().view(B, 1),
                                     self.tok_emb_cond.weight, self.pos_emb_cond.view(-1, C), self.tok_emb_code.weight,
                                     pos_code.contiguous().view(1, C))
-            for li, block in enumerate(self.blocks):
-                att = block.attn
-                h = Fn.LayerNormFn.apply(x, block.ln1.weight, block.ln1.bias, False)
-                mixed = ops.time_mix_fwd(h, att.time_mix.view(-1), 1)
-                w, b = att.packed_qkv()
-                qkv = _linear(mixed, w, b)
-                o = ops.decode_attention(qkv, past["k"][li], past["v"][li], heads, hs, pos, scale)
-                x = _linear(o, att.proj.weight, att.proj.bias, x)
-                x = block.mlp.core(Fn.LayerNormFn.apply(x, block.ln2.weight, block.ln2.bias, False), res=x)
-            past["len"] = pos + 1
+            x = _cached_step(self.blocks, x, past, heads, hs)
             x = Fn.LayerNormFn.apply(x, self.layer_norm.weight, self.layer_norm.bias, False)
         logits = _linear(x, self.head.weight, None)
         return logits, past
+
+
+class RQTransformer(nn.Module):
+    """reference stage2/layers.py:306-547: a spatial transformer over the code positions and a depth transformer over the D
+    residual codes of each position.  Reproduces what the reference computes, quirks included: the code embeddings are
+    prefix sums over the channel axis (`cumsum(-1)`, :378), the sampler embeds codes as sums over depth (:502, :535) and
+    applies `ln_depth` twice on depth step 0 (:531, :542).  Limits of the kernels underneath, raised at construction: head
+    sizes 32 / 64 (spatial and depth), `embed_dim` <= 2048 and a multiple of 64, `vocab_img_size` % 64 == 0,
+    2 <= `depth_num_tokens` <= 16."""
+
+    def __init__(self, vocab_cond_size: int, vocab_img_size: int, embed_dim: int, cond_num_tokens: int, img_num_tokens: int,
+                 depth_num_tokens: int, spatial_n_heads: int, depth_n_heads: int, spatial_n_layers: int, depth_n_layers: int,
+                 mlp_bias: bool = True, attn_bias: bool = True) -> None:
+        super().__init__()
+        if vocab_img_size % 64:
+            raise NotImplementedError(f"b200vq stage 2: vocab_img_size must be a multiple of 64 (got {vocab_img_size})")
+        if not 2 <= depth_num_tokens <= 16:
+            # the short-sequence attention kernel holds a whole depth sequence per warp
+            raise NotImplementedError(f"b200vq stage 2: depth_num_tokens must be in 2..16 (got {depth_num_tokens})")
+        _check_kernel_limits(embed_dim, spatial_n_heads)
+        _check_kernel_limits(embed_dim, depth_n_heads)
+        self.img_num_tokens = img_num_tokens
+        self.depth_num_tokens = depth_num_tokens
+        self.vocab_img_size = vocab_img_size
+        self.tok_emb_cond = nn.Embedding(vocab_cond_size, embed_dim)
+        self.pos_emb_cond = nn.Parameter(torch.rand(1, cond_num_tokens, embed_dim))
+        self.tok_emb_code = nn.Embedding(vocab_img_size, embed_dim)
+        self.pos_emb_code = nn.Parameter(torch.rand(1, img_num_tokens, embed_dim))
+        self.pos_emb_depth = nn.Parameter(torch.rand(1, depth_num_tokens - 1, embed_dim))
+        self.spatial_transformer = nn.Sequential(*[Block(ctx_len=cond_num_tokens + img_num_tokens, cond_len=cond_num_tokens,
+                                                         embed_dim=embed_dim, n_heads=spatial_n_heads, mlp_bias=mlp_bias,
+                                                         attn_bias=attn_bias) for _ in range(spatial_n_layers)])
+        self.depth_transformer = nn.Sequential(*[Block(ctx_len=depth_num_tokens, cond_len=0, embed_dim=embed_dim,
+                                                       n_heads=depth_n_heads, mlp_bias=mlp_bias, attn_bias=attn_bias)
+                                                 for _ in range(depth_n_layers)])
+        for block in self.depth_transformer:
+            block.attn.short_seq = True
+        self.ln_spatial = nn.LayerNorm(embed_dim)
+        self.ln_depth = nn.LayerNorm(embed_dim)
+        self.head = nn.Linear(embed_dim, vocab_img_size, bias=False)
+        self.apply(self._init_weights)
+
+    _init_weights = GPT._init_weights
+
+    def forward(self, codes: torch.LongTensor, conds: torch.LongTensor) -> torch.FloatTensor:
+        """reference stage2/layers.py:370-395: codes [B, T, D], conds [B, Tc] -> logits [B*T, D, vocab_img_size]"""
+        D = codes.shape[-1]
+        codes = codes.reshape(codes.shape[0], -1, D).contiguous()
+        conds = conds.contiguous()
+        B, Tc = conds.shape
+        T = codes.shape[1]
+        assert D == self.depth_num_tokens and T == self.pos_emb_code.shape[1] and Tc == self.pos_emb_cond.shape[1], \
+            "codes / conds must be [B, img_num_tokens, depth_num_tokens] / [B, cond_num_tokens] (the positional tables are added whole)"
+        x = RQEmbedFn.apply(conds, codes, self.tok_emb_cond.weight, self.pos_emb_cond, self.tok_emb_code.weight, self.pos_emb_code)
+        for block in self.spatial_transformer:
+            x = block.run(x, B, Tc + T)
+        x = Fn.LayerNormFn.apply(x, self.ln_spatial.weight, self.ln_spatial.bias, False)
+        h = RowWindowFn.apply(x, B, Tc + T, Tc - 1, T)                 # positions cond-1 .. Tc+T-2 (:386)
+        v = RQDepthInputFn.apply(h, codes, self.tok_emb_code.weight, self.pos_emb_depth)
+        for block in self.depth_transformer:
+            v = block.run(v, B * T, D)
+        v = Fn.LayerNormFn.apply(v, self.ln_depth.weight, self.ln_depth.bias, False)
+        return _linear(v, self.head.weight, None).view(B * T, D, -1)
+
+    # ------------------------------------------------------------------------------------------ sampling
+    @torch.no_grad()
+    def sample(self, conds: torch.LongTensor, top_k: Optional[float] = None, top_p: Optional[float] = None,
+               softmax_temperature: float = 1.0, use_fp16: bool = True) -> Tuple[torch.FloatTensor, torch.LongTensor]:
+        """reference stage2/layers.py:397-477 -> (logits [B*T, D, vocab], codes [B, T, D]).  The filtering and the draw are the
+        reference's torch calls; the steps run in libb200vq.so with one preallocated KV cache per layer per transformer (the
+        depth caches are [B, D, C], reused at every position).  `use_fp16` is accepted and ignored, as in GPT.sample."""
+        B, T, D, S = conds.shape[0], self.img_num_tokens, self.depth_num_tokens, self.vocab_img_size
+        past = depth_past = codes = logits = None
+        for i in range(T):
+            if codes is None:
+                hidden, past = self.sample_spatial_step(None, conds, None, use_fp16, None)
+            else:
+                hidden, past = self.sample_spatial_step(codes[:, -D:], conds, self.pos_emb_code[:, i - 1:i, :], use_fp16, past)
+            last_len = 0 if codes is None else codes.shape[-1]
+            for d in range(D):
+                if d == 0:
+                    logits_, depth_past = self.sample_depth_step(None, hidden, None, use_fp16, depth_past)
+                else:
+                    logits_, depth_past = self.sample_depth_step(codes[:, last_len:], hidden, self.pos_emb_depth[:, d - 1:d, :],
+                                                                 use_fp16, depth_past)
+                logits_ = logits_.to(dtype=torch.float32) / softmax_temperature
+                idx = _filter_and_draw(logits_, top_k, top_p)
+                codes = idx if codes is None else torch.cat([codes, idx], axis=1)
+                logits = logits_ if logits is None else torch.cat([logits, logits_], axis=1)
+        return logits.view(B * T, D, S), codes.view(B, T, D)
+
+    def _heads(self, blocks) -> Tuple[int, int]:
+        C = self.head.weight.shape[1]
+        heads = blocks[0].attn.n_heads if len(blocks) else 1
+        return heads, C // heads
+
+    @torch.no_grad()
+    def sample_spatial_step(self, codes, conds, pos_code, use_fp16: bool = True, past=None):
+        """reference stage2/layers.py:479-512 -> (hidden [B, 1, C] = ln_spatial of the newest row, past).  codes: the previous
+        position's D codes [B, D] (None on the first step), embedded as their sum over depth plus pos_code (:501-502).
+        `past` is this implementation's cache object: per-layer key / value buffers [B, Tc + T, C] and the rows filled."""
+        C = self.head.weight.shape[1]
+        heads, hs = self._heads(self.spatial_transformer)
+        if codes is None:
+            assert past is None
+            conds = conds.contiguous()
+            B, Tc = conds.shape
+            empty = torch.empty(B, 0, dtype=torch.int64, device=conds.device)
+            x = ops.token_embed_fwd(conds, empty, self.tok_emb_cond.weight, self.pos_emb_cond.view(Tc, C), self.tok_emb_code.weight,
+                                    self.pos_emb_code.view(-1, C))
+            x, past = _cached_prefix(self.spatial_transformer, x, B, Tc, Tc + self.img_num_tokens, heads, hs)
+            x = Fn.LayerNormFn.apply(x, self.ln_spatial.weight, self.ln_spatial.bias, False)
+            x = ops.copy_rows(x, B, Tc, 1, Tc - 1, 0, 1)
+        else:
+            assert past is not None
+            B = codes.shape[0]
+            x = ops.code_sum_embed(codes, codes.shape[1], self.tok_emb_code.weight, pos_code.contiguous().view(C))
+            x = _cached_step(self.spatial_transformer, x, past, heads, hs)
+            x = Fn.LayerNormFn.apply(x, self.ln_spatial.weight, self.ln_spatial.bias, False)
+        return x.view(B, 1, C), past
+
+    @torch.no_grad()
+    def sample_depth_step(self, codes, hidden, pos_depth, use_fp16: bool = True, past=None):
+        """reference stage2/layers.py:514-547 -> (logits [B, vocab], past).  codes None: depth step 0 on `hidden`, with
+        ln_depth applied twice (:531, :542); a `past` handed in then is a previous position's depth cache ([B, D, C] per
+        layer), whose buffers are reused (step 0 writes row 0 and reads nothing beyond it).  Otherwise codes [B, d] are this position's codes so far,
+        embedded as their sum plus pos_depth (:534-535)."""
+        C = self.head.weight.shape[1]
+        heads, hs = self._heads(self.depth_transformer)
+        ln = lambda t: Fn.LayerNormFn.apply(t, self.ln_depth.weight, self.ln_depth.bias, False)   # noqa: E731
+        if codes is None:
+            x = hidden.contiguous().view(-1, C)
+            if past is None:
+                B = x.shape[0]
+                past = {"k": [torch.zeros(B, self.depth_num_tokens, C, device=x.device) for _ in self.depth_transformer],
+                        "v": [torch.zeros(B, self.depth_num_tokens, C, device=x.device) for _ in self.depth_transformer]}
+            past["len"] = 0          # one token attending to itself: decode_attention at row 0
+            x = ln(_cached_step(self.depth_transformer, x, past, heads, hs))
+        else:
+            assert past is not None
+            x = ops.code_sum_embed(codes, codes.shape[1], self.tok_emb_code.weight, pos_depth.contiguous().view(C))
+            x = _cached_step(self.depth_transformer, x, past, heads, hs)
+        x = ln(x)
+        return _linear(x, self.head.weight, None), past

@@ -234,6 +234,48 @@ int b200vq_copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, 
 int b200vq_decode_attention(const float* qkv, float* cache_k, float* cache_v, float* out, int B, int heads, int hs, int Tmax,
                             int pos, float scale, void* stream);
 
+/* ---- stage-2 RQTransformer (reference enhancing/modules/stage2/layers.py:306-547) ---------------------------------------
+ * short_attention: the depth transformer's attention core -- nseq independent sequences of D tokens (1 <= D <= 16), the
+ *   packed qkv [nseq*D, 3*heads*hs] of b200vq_attention_causal_fwd (q | k | v thirds, head h at columns h*hs) -> out
+ *   [nseq*D, heads*hs]; the mask of b200vq_attention_causal_fwd (k <= max(q, cond_len - 1)); hs 32 or 64, heads*hs <= 2048.
+ *   fp32 FMA arithmetic and an fp32 softmax on every data path.  bwd recomputes the scores from qkv and writes every
+ *   element of dqkv [nseq*D, 3*heads*hs] (no lse / out / delta needed, no atomics: the same bits on every run).  Both
+ *   are persistent grid-stride kernels: b200vq_set_sm_limit caps their grid at that many CTAs (the results do not
+ *   depend on the grid).
+ * rq_embed: the spatial input x [B, Tc + T, C] of layers.py:374-384: rows t < Tc are Wc[conds[b, t]] + pos_c[t]; row Tc + t is
+ *   cumsum over the channels of Wi[codes[b, t, D-1]] (scanned in fp64, rounded once: torch's CPU cumsum bit for bit) +
+ *   pos_i[t].  conds int64 [B, Tc], codes int64 [B, T, D].  bwd: gWc / gWi zero-filled then accumulated with float
+ *   atomics (gWi as the reverse channel scan of the scattered rows; with Tc == 0 a non-NULL gWc comes out all zero),
+ *   gpos_c [Tc, C] / gpos_i [T, C] = sums over the batch in a fixed order.  bwd_deterministic: the same with gWc / gWi summed in a fixed order (the sort and segmented sum of
+ *   b200vq_token_embed_bwd_deterministic) -- bit-reproducible whatever the SM count; workspace from its query.
+ * rq_depth_input: the depth input v [nseq*D, C] of layers.py:388-391 (nseq = B*T): v[s, 0] = h[s] (h [nseq, C]);
+ *   v[s, d] = cumsum over the channels of Wi[codes[s, d-1]] + pos_d[d-1] for d >= 1 (codes int64 [nseq, D], pos_d
+ *   [D-1, C]).  bwd: gh [nseq, C] = the row-0 gradients, gWi as in rq_embed_bwd, gpos_d [D-1, C] = sums over the sequences
+ *   in a fixed order.  bwd_deterministic as for rq_embed.
+ * code_sum_embed: out[b] = sum_{j < n} Wi[codes[b*ld + j]] + pos (pos one [C] row): the inputs of the sampling steps,
+ *   layers.py:501-502 (the previous position's D codes) and :534-535 (this position's codes so far). */
+int b200vq_short_attention_fwd(const float* qkv, float* out, long long nseq, int D, int heads, int hs, int cond_len, float scale,
+                               void* stream);
+int b200vq_short_attention_bwd(const float* qkv, const float* dout, float* dqkv, long long nseq, int D, int heads, int hs, int cond_len,
+                               float scale, void* stream);
+int b200vq_rq_embed_fwd(const long long* conds, const long long* codes, const float* Wc, const float* pos_c, const float* Wi,
+                        const float* pos_i, float* x, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* stream);
+int b200vq_rq_embed_bwd(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c, float* gWi,
+                        float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* stream);
+size_t b200vq_rq_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int T, int D, int C, int Vc, int Vi);
+int b200vq_rq_embed_bwd_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                      float* gWi, float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* workspace,
+                                      size_t ws_bytes, void* stream);
+int b200vq_rq_depth_input_fwd(const float* h, const long long* codes, const float* Wi, const float* pos_d, float* v, long long nseq,
+                              int D, int C, int Vi, void* stream);
+int b200vq_rq_depth_input_bwd(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq, int D, int C,
+                              int Vi, void* stream);
+size_t b200vq_rq_depth_input_bwd_deterministic_workspace_bytes(long long nseq, int D, int C, int Vi);
+int b200vq_rq_depth_input_bwd_deterministic(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq,
+                                            int D, int C, int Vi, void* workspace, size_t ws_bytes, void* stream);
+int b200vq_code_sum_embed(const long long* codes, long long ld, int n, const float* Wi, const float* pos, float* out, int B, int C, int Vi,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif
