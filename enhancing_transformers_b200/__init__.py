@@ -12,28 +12,30 @@ from .functional import get_precision, invalidate_shadows, set_precision  # noqa
 from .layers import (Attention, FeedForward, PosQuantLinear, PreNorm, QuantLinear, Transformer, ViTDecoder, ViTEncoder,  # noqa: F401
                      sincos_table)
 from .parallel import FlatGradients, allreduce_gradients  # noqa: F401
-from .quantizers import BaseQuantizer, GumbelQuantizer, VectorQuantizer  # noqa: F401
+from .quantizers import BaseQuantizer, EMAVectorQuantizer, GumbelQuantizer, VectorQuantizer  # noqa: F401
 from . import stage2  # noqa: F401
 from .stage2 import GPT, RQTransformer  # noqa: F401
 
 __version__ = "0.2.0"
-__all__ = ["ViTEncoder", "ViTDecoder", "VectorQuantizer", "GumbelQuantizer", "BaseQuantizer", "Transformer", "Attention", "FeedForward",
+__all__ = ["ViTEncoder", "ViTDecoder", "VectorQuantizer", "EMAVectorQuantizer", "GumbelQuantizer", "BaseQuantizer", "Transformer", "Attention", "FeedForward",
            "PreNorm", "QuantLinear", "PosQuantLinear", "fuse_post_quant_pos", "detach_discriminator_forward", "GPT", "RQTransformer", "stage2", "patch", "patch_stage2", "install_as_reference_modules", "fuse_quant_linears", "set_precision",
            "get_precision", "invalidate_shadows", "allreduce_gradients", "FlatGradients", "ops", "functional", "configs"]
 
 _REF_PKG = "enhancing.modules.stage1"
 
 
-def patch(vitvqgan_module=None):
+def patch(vitvqgan_module=None, ema=False):
     """Rebind the three names ``ViTVQ.__init__`` looks up at construction time
     (reference vitvqgan.py:20-21,35-37).  Pass the already-imported module, or leave None to
-    import ``enhancing.modules.stage1.vitvqgan``.  The reference file itself is not edited."""
+    import ``enhancing.modules.stage1.vitvqgan``.  The reference file itself is not edited.
+    ema=True binds ``VectorQuantizer`` to `EMAVectorQuantizer`: the YAML's ``quantizer:`` block, which ``ViTVQ`` splats
+    into the constructor (vitvqgan.py:37), may then also set ``decay`` and ``eps``."""
     if vitvqgan_module is None:
         import importlib
         vitvqgan_module = importlib.import_module(_REF_PKG + ".vitvqgan")
     vitvqgan_module.Encoder = ViTEncoder
     vitvqgan_module.Decoder = ViTDecoder
-    vitvqgan_module.VectorQuantizer = VectorQuantizer
+    vitvqgan_module.VectorQuantizer = EMAVectorQuantizer if ema else VectorQuantizer
     vitvqgan_module.GumbelQuantizer = GumbelQuantizer      # ViTVQGumbel (vitvqgan.py:147-176)
     _wrap_vitvq_init(vitvqgan_module)
     return vitvqgan_module

@@ -41,6 +41,9 @@ _SIGNATURES = {
     "b200vq_vq_bwd_deterministic_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i]),
     "b200vq_vq_bwd_deterministic": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_fl, c_i, c_f, c_sz, c_f]),
     "b200vq_vq_embed": (c_i, [c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_f]),
+    "b200vq_vq_fwd_ema_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i, c_i]),
+    "b200vq_vq_fwd_ema": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_fl, c_i, c_i, c_f, c_sz, c_f]),
+    "b200vq_vq_ema_update": (c_i, [c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_fl, c_fl, c_f]),
     "b200vq_patchify": (c_i, [c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_unpatchify": (c_i, [c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_i, c_f]),
     "b200vq_colsum_workspace_bytes": (c_sz, [c_i]),

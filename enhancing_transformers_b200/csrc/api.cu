@@ -87,6 +87,10 @@ int vq_embed(const float*, const long long*, float*, int, int, int, int, int, cu
 size_t vq_bwd_deterministic_workspace_bytes(int, int, int, int);
 int vq_backward_deterministic(const float*, const float*, const long long*, const float*, const float*, float*, float*, int, int, int,
                               int, int, float, int, void*, size_t, cudaStream_t);
+size_t vq_fwd_ema_workspace_bytes(int, int, int, int, int);
+int vq_forward_ema(const float*, const float*, float*, long long*, float*, float*, float*, int, int, int, int, float, int, int, void*,
+                   size_t, cudaStream_t);
+int vq_ema_update(const float*, const float*, float*, float*, float*, int, int, float, float, cudaStream_t);
 int patchify(const float*, float*, int, int, int, int, int, int, int, cudaStream_t);
 int unpatchify(const float*, const float*, float*, int, int, int, int, int, int, cudaStream_t);
 size_t colsum_workspace_bytes(int);
@@ -234,6 +238,18 @@ int b200vq_vq_bwd_deterministic(const float* z, const float* E, const long long*
 int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
                     void* stream) {
   return vq_embed(E, codes, out, M, K, D, depth, use_norm, S(stream));
+}
+size_t b200vq_vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int deterministic) {
+  return vq_fwd_ema_workspace_bytes(M, K, D, depth, deterministic);
+}
+int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, long long* idx, float* loss, float* counts, float* sums, int M, int K,
+                      int D, int depth, float beta, int use_norm, int deterministic, void* workspace, size_t ws_bytes, void* stream) {
+  return vq_forward_ema(z, E, out, idx, loss, counts, sums, M, K, D, depth, beta, use_norm, deterministic, workspace, ws_bytes,
+                        S(stream));
+}
+int b200vq_vq_ema_update(const float* counts, const float* sums, float* cluster_size, float* embed_avg, float* weight, int K, int D,
+                         float decay, float eps, void* stream) {
+  return vq_ema_update(counts, sums, cluster_size, embed_avg, weight, K, D, decay, eps, S(stream));
 }
 int b200vq_patchify(const float* img, float* patches, int B, int C, int H, int W, int ph, int pw, int round_out, void* stream) {
   return patchify(img, patches, B, C, H, W, ph, pw, round_out, S(stream));

@@ -9,6 +9,9 @@
 //             depth loop (:42-57) runs inside the kernel.  The [tokens, n_embed] distance
 //             matrix the reference materialises never exists.
 //   vq_loss : deterministic reduction of the per-CTA partial sums into the scalar loss.
+//   EMA codebook (EMAVectorQuantizer): vq_fwd with kStats != 0 also gathers, per code k, the count n_k and the sum s_k of
+//             the vectors the lookup compared (a per-CTA shared-memory table flushed once per depth, or per-entry rows
+//             summed by scatter_det.cu in a fixed order); vq_ema_* apply the update to the codebook on the device.
 //   vq_bwd  : closed-form gradients (see oracle/vitvq_oracle.py:vq_backward_np).  The codebook gradient is scattered with
 //             float atomics (vq_bwd_kernel) or, on request, stored per entry and summed in a fixed order
 //             (vq_bwd_contrib_kernel + scatter_det.cu): bit-reproducible.
@@ -79,13 +82,53 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+// EMA statistics of one CTA and one depth step.  A CTA looks up 128 tokens per depth, so it meets at most 128 distinct
+// codes: a 128-slot open-addressing table keyed by code never overflows.  Counts are integers (order-independent); the
+// float sums of kVqStatsAtomic are shared-memory atomics here and one global atomic per (live slot, column) at the flush.
+constexpr int kVqStatsOff = 0, kVqStatsAtomic = 1, kVqStatsDeterministic = 2;
+constexpr int kVqStatSlots = 128;
+struct VqStatTable {
+  int keys[kVqStatSlots];
+  int cnt[kVqStatSlots];
+  float acc[kVqStatSlots][kVqD];
+};
+__device__ __forceinline__ void vq_stat_clear(VqStatTable& st, int tid) {
+  for (int i = tid; i < kVqStatSlots; i += kVqThreads) { st.keys[i] = -1; st.cnt[i] = 0; }
+#pragma unroll 1
+  for (int i = tid; i < kVqStatSlots * kVqD; i += kVqThreads) (&st.acc[0][0])[i] = 0.f;
+}
+// every lane of the warp calls this (the slot travels by shuffle); dead tokens (live == false) add nothing
+template <int kStats>
+__device__ __forceinline__ void vq_stat_add(VqStatTable& st, int code, int part, bool live, const float4& x) {
+  int slot = -1;
+  if (part == 0 && live) {
+    unsigned h = ((unsigned)code * 2654435761u) >> 25;
+#pragma unroll 1
+    for (int probe = 0; probe < kVqStatSlots; ++probe) {
+      const int old = atomicCAS(&st.keys[h], -1, code);
+      if (old == -1 || old == code) { slot = (int)h; break; }
+      h = (h + 1) & (kVqStatSlots - 1);
+    }
+    atomicAdd(&st.cnt[slot], 1);
+  }
+  slot = __shfl_sync(0xffffffffu, slot, (threadIdx.x & 31) & ~7);
+  if (kStats == kVqStatsAtomic && slot >= 0) {
+    float* dst = &st.acc[slot][part * 4];
+    atomicAdd(dst + 0, x.x); atomicAdd(dst + 1, x.y); atomicAdd(dst + 2, x.z); atomicAdd(dst + 3, x.w);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // z [M,32] fp32; EnT [32][K]; ee [K]; E [K,32] (un-normalised codebook, gathered for the winner)
 // out [M,32]; idx [M,depth] int64; loss_part [depth][gridDim.x]
+// kStats != 0 (EMA statistics): counts [K] int (accumulated); kVqStatsAtomic: sums [K,32] (accumulated);
+// kVqStatsDeterministic: contrib [M*depth, 32] receives the compared vector of entry m*depth + t
+template <int kStats>
 __global__ void __launch_bounds__(kVqThreads, 2)
 vq_fwd_kernel(const float* __restrict__ z, const float* __restrict__ EnT, const float* __restrict__ ee,
               const float* __restrict__ E, float* __restrict__ out, long long* __restrict__ idx_out,
-              float* __restrict__ loss_part, int M, int K, int depth, int use_norm) {
+              float* __restrict__ loss_part, int M, int K, int depth, int use_norm, int* __restrict__ counts,
+              float* __restrict__ sums, float* __restrict__ contrib) {
   extern __shared__ __align__(16) uint8_t vq_smem[];
   float (*zT)[kVqTileM] = reinterpret_cast<float (*)[kVqTileM]>(vq_smem);                       // normalised residual, transposed
   float (*eT)[kVqD][kVqTileN] = reinterpret_cast<float (*)[kVqD][kVqTileN]>(vq_smem + sizeof(float) * kVqD * kVqTileM);  // chunk ring
@@ -96,6 +139,7 @@ vq_fwd_kernel(const float* __restrict__ z, const float* __restrict__ EnT, const 
   // residual / accumulated-code state of the depth loop, parked in shared memory while the distance loop runs: it is only
   // touched in phases A and C, and keeping its 32 registers live across phase B spilled the 8x8 accumulator tile
   float4* park = reinterpret_cast<float4*>(red_s + 8);          // [8][256]: rreg[ps] at ps*256 + tid, acc[ps] at (4+ps)*256 + tid
+  VqStatTable* st = reinterpret_cast<VqStatTable*>(park + 8 * kVqThreads);   // kStats != 0 only
 
   const int tid = threadIdx.x;
   const int m0 = blockIdx.x * kVqTileM;
@@ -112,6 +156,7 @@ vq_fwd_kernel(const float* __restrict__ z, const float* __restrict__ EnT, const 
     park[(4 + ps) * kVqThreads + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   const int nchunks = (K + kVqTileN - 1) / kVqTileN;
+  if constexpr (kStats != kVqStatsOff) vq_stat_clear(*st, tid);   // first used in phase C, after phase B's barriers
 
   for (int t = 0; t < depth; ++t) {
     // ---- phase A: normalise the residual, stage it transposed -------------------------------
@@ -224,6 +269,34 @@ vq_fwd_kernel(const float* __restrict__ z, const float* __restrict__ EnT, const 
     lsum = warp_sum(lsum);
     if ((tid & 31) == 0) red_s[tid >> 5] = lsum;
     __syncthreads();
+    if constexpr (kStats != kVqStatsOff) {
+      // EMA statistics of this depth.  zT still holds the vectors the lookup compared (phase C recomputed the same values)
+      // and best_s the codes: reading them here, behind the barrier, keeps phase C's registers as they are.
+#pragma unroll 1
+      for (int ps = 0; ps < 4; ++ps) {
+        const int lt = ps * 32 + (tid >> 3);
+        const int tok = m0 + lt;
+        int code = best_s[lt];
+        if (code >= K) code = 0;   // as phase C
+        const float4 x = make_float4(zT[part * 4 + 0][lt], zT[part * 4 + 1][lt], zT[part * 4 + 2][lt], zT[part * 4 + 3][lt]);
+        vq_stat_add<kStats>(*st, code, part, tok < M, x);
+        if (kStats == kVqStatsDeterministic && tok < M)
+          *reinterpret_cast<float4*>(contrib + ((size_t)tok * depth + t) * kVqD + part * 4) = x;
+      }
+      __syncthreads();
+      // flush the table, then clear it for the next depth (whose statistics follow phase B's barriers)
+#pragma unroll 1
+      for (int i = tid; i < kVqStatSlots * kVqD; i += kVqThreads) {
+        const int slot = i / kVqD, col = i % kVqD;
+        const int key = st->keys[slot];
+        if (key >= 0) {
+          if (kStats == kVqStatsAtomic) atomicAdd(sums + (size_t)key * kVqD + col, st->acc[slot][col]);
+          if (col == 0) atomicAdd(counts + key, st->cnt[slot]);
+        }
+      }
+      __syncthreads();
+      vq_stat_clear(*st, tid);
+    }
     if (tid == 0) {
       float s = 0.f;
       for (int w = 0; w < kVqThreads / 32; ++w) s += red_s[w];
@@ -250,6 +323,8 @@ vq_fwd_kernel(const float* __restrict__ z, const float* __restrict__ EnT, const 
 }
 
 // loss = mean_t( beta * m_t + m_t ),  m_t = sum_t / (M * D)      (quantizers.py:56-57,89-90)
+// kEma: loss = mean_t( beta * m_t ) -- the EMA codebook has no codebook term
+template <bool kEma>
 __global__ void vq_loss_kernel(const float* __restrict__ loss_part, int nparts, int depth, float inv_count, float beta,
                                float* __restrict__ loss_out) {
   __shared__ float red[32];
@@ -264,7 +339,8 @@ __global__ void vq_loss_kernel(const float* __restrict__ loss_part, int nparts, 
       float a = 0.f;
       for (int w = 0; w < (int)(blockDim.x >> 5); ++w) a += red[w];
       const float m = a * inv_count;
-      total += beta * m + m;
+      if constexpr (kEma) total += beta * m;
+      else total += beta * m + m;
     }
     __syncthreads();
   }
@@ -464,10 +540,11 @@ int vq_forward(const float* z, const float* E, float* out, long long* idx, float
   const int nblk = (M + kVqTileM - 1) / kVqTileM;
   vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
   B200_LAUNCH_OK("vq_prep_kernel");
-  B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel, kVqSmemBytes);
-  vq_fwd_kernel<<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm);
+  B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsOff>, kVqSmemBytes);
+  vq_fwd_kernel<kVqStatsOff><<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
+                                                                         nullptr, nullptr, nullptr);
   B200_LAUNCH_OK("vq_fwd_kernel");
-  vq_loss_kernel<<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)kVqD), beta, loss);
+  vq_loss_kernel<false><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)kVqD), beta, loss);
   B200_LAUNCH_OK("vq_loss_kernel");
   return 0;
 }
@@ -518,6 +595,134 @@ int vq_embed(const float* E, const long long* codes, float* out, int M, int K, i
   B200_CHECK_ARG(M > 0 && M % 4 == 0 && depth >= 1, "vq_embed: bad sizes");
   vq_embed_kernel<<<(M * 8 + 255) / 256, 256, 0, stream>>>(E, codes, out, M, K, depth, use_norm);
   B200_LAUNCH_OK("vq_embed_kernel");
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// EMA codebook (van den Oord et al. 2017, appendix A.1, in the form of Taming Transformers' EMAVectorQuantizer)
+__global__ void vq_counts_to_float_kernel(const int* __restrict__ icounts, float* __restrict__ counts, int K) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < K) counts[k] = (float)icounts[k];    // exact: a count never exceeds M * depth < 2^24 (checked by the host)
+}
+
+// cluster_size <- decay * cluster_size + (1 - decay) * n;  embed_avg <- decay * embed_avg + (1 - decay) * s
+__global__ void vq_ema_accumulate_kernel(const float* __restrict__ counts, const float* __restrict__ sums,
+                                         float* __restrict__ cluster_size, float* __restrict__ embed_avg, int K, float decay,
+                                         float one_minus_decay) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= K * kVqD) return;
+  embed_avg[i] = decay * embed_avg[i] + one_minus_decay * sums[i];
+  if (i % kVqD == 0) cluster_size[i / kVqD] = decay * cluster_size[i / kVqD] + one_minus_decay * counts[i / kVqD];
+}
+
+// weight_k = embed_avg_k / ((cluster_size_k + eps) / (N + K eps) * N),  N = sum_k cluster_size_k.  Every CTA sums N itself
+// in the same fixed order (strided per thread, then the warps' partials in order), so N has the same bits in every CTA
+// and on every run, and no grid-wide barrier or scratch is needed.
+constexpr int kVqEmaRowsPerCta = 64;
+__global__ void __launch_bounds__(256)
+vq_ema_weight_kernel(const float* __restrict__ cluster_size, const float* __restrict__ embed_avg, float* __restrict__ weight, int K,
+                     float eps, float k_eps) {
+  __shared__ float red[8];
+  float s = 0.f;
+  for (int k = threadIdx.x; k < K; k += 256) s += cluster_size[k];
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  float N = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) N += red[w];
+  const float denom = N + k_eps;
+  const int r0 = blockIdx.x * kVqEmaRowsPerCta;
+  for (int i = threadIdx.x; i < kVqEmaRowsPerCta * kVqD; i += 256) {
+    const int k = r0 + i / kVqD;
+    if (k >= K) break;
+    const float smoothed = (cluster_size[k] + eps) / denom * N;
+    weight[(size_t)k * kVqD + i % kVqD] = embed_avg[(size_t)k * kVqD + i % kVqD] / smoothed;
+  }
+}
+
+static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+
+// [EnT | ee | loss parts] as vq_forward, [int counts K], deterministic: [contributions M*depth x 32 | scatter scratch]
+size_t vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int deterministic) {
+  if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || D != kVqD) return 0;
+  size_t b = align256(vq_workspace_bytes(M, K, depth)) + align256((size_t)K * sizeof(int));
+  if (deterministic) {
+    const long long n = (long long)M * depth;
+    b += align256((size_t)n * kVqD * sizeof(float)) + scatter_det_workspace_bytes(n, K, kVqD, kScatterRunVq);
+  }
+  return b;
+}
+
+int vq_forward_ema(const float* z, const float* E, float* out, long long* idx, float* loss, float* counts, float* sums, int M, int K,
+                   int D, int depth, float beta, int use_norm, int deterministic, void* workspace, size_t ws_bytes,
+                   cudaStream_t stream) {
+  B200_CHECK_ARG(D == kVqD, "vq_fwd_ema: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq_fwd_ema: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
+  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq_fwd_ema: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
+  B200_CHECK_ARG(z && E && out && idx && loss && workspace, "vq_fwd_ema: null pointer argument");
+  B200_CHECK_ARG((counts == nullptr) == (sums == nullptr), "vq_fwd_ema: counts and sums must both be given or both be NULL");
+  B200_CHECK_ARG((long long)M * depth < (1ll << 24), "vq_fwd_ema: M * depth must be below 2^24 (fp32 counts stay exact)");
+  B200_CHECK_ARG(ws_bytes >= vq_fwd_ema_workspace_bytes(M, K, D, depth, deterministic), "vq_fwd_ema: workspace too small");
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  float* EnT = reinterpret_cast<float*>(ws);
+  float* ee = EnT + (size_t)kVqD * K;
+  float* part = ee + K;
+  ws += align256(vq_workspace_bytes(M, K, depth));
+  int* icounts = reinterpret_cast<int*>(ws);
+  ws += align256((size_t)K * sizeof(int));
+  float* contrib = reinterpret_cast<float*>(ws);
+  const long long n = (long long)M * depth;
+  const int nblk = (M + kVqTileM - 1) / kVqTileM;
+  const bool stats = counts != nullptr;
+  vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
+  B200_LAUNCH_OK("vq_prep_kernel");
+  constexpr size_t stat_smem = kVqSmemBytes + sizeof(VqStatTable);
+  if (!stats) {
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsOff>, kVqSmemBytes);
+    vq_fwd_kernel<kVqStatsOff><<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
+                                                                           nullptr, nullptr, nullptr);
+  } else {
+    B200_CUDA_OK(cudaMemsetAsync(icounts, 0, (size_t)K * sizeof(int), stream));
+    if (deterministic) {
+      B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsDeterministic>, stat_smem);
+      vq_fwd_kernel<kVqStatsDeterministic><<<nblk, kVqThreads, stat_smem, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth,
+                                                                                    use_norm, icounts, nullptr, contrib);
+    } else {
+      B200_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)K * kVqD * sizeof(float), stream));
+      B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsAtomic>, stat_smem);
+      vq_fwd_kernel<kVqStatsAtomic><<<nblk, kVqThreads, stat_smem, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
+                                                                             icounts, sums, nullptr);
+    }
+  }
+  B200_LAUNCH_OK("vq_fwd_kernel");
+  vq_loss_kernel<true><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)kVqD), beta, loss);
+  B200_LAUNCH_OK("vq_loss_kernel");
+  if (!stats) return 0;
+  if (deterministic) {
+    uint8_t* scratch = reinterpret_cast<uint8_t*>(contrib) + align256((size_t)n * kVqD * sizeof(float));
+    const size_t used = (size_t)(scratch - static_cast<uint8_t*>(workspace));
+    const int rc = scatter_rows_det<kScatterRunVq>(idx, n, K, contrib, n, 0, 0, kVqD, sums, scratch, ws_bytes - used, stream);
+    if (rc != 0) return rc;
+  }
+  vq_counts_to_float_kernel<<<(K + 255) / 256, 256, 0, stream>>>(icounts, counts, K);
+  B200_LAUNCH_OK("vq_counts_to_float_kernel");
+  return 0;
+}
+
+int vq_ema_update(const float* counts, const float* sums, float* cluster_size, float* embed_avg, float* weight, int K, int D,
+                  float decay, float eps, cudaStream_t stream) {
+  B200_CHECK_ARG(D == kVqD, "vq_ema_update: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(K > 0, "vq_ema_update: n_embed must be positive (got %d)", K);
+  B200_CHECK_ARG(counts && sums && cluster_size && embed_avg && weight, "vq_ema_update: null pointer argument");
+  B200_CHECK_ARG(decay >= 0.f && decay <= 1.f, "vq_ema_update: decay must be in [0, 1] (got %g)", (double)decay);
+  B200_CHECK_ARG(eps >= 0.f, "vq_ema_update: eps must be non-negative (got %g)", (double)eps);
+  vq_ema_accumulate_kernel<<<(K * kVqD + 255) / 256, 256, 0, stream>>>(counts, sums, cluster_size, embed_avg, K, decay,
+                                                                       (float)(1.0 - (double)decay));
+  B200_LAUNCH_OK("vq_ema_accumulate_kernel");
+  vq_ema_weight_kernel<<<(K + kVqEmaRowsPerCta - 1) / kVqEmaRowsPerCta, 256, 0, stream>>>(cluster_size, embed_avg, weight, K, eps,
+                                                                                        (float)((double)K * (double)eps));
+  B200_LAUNCH_OK("vq_ema_weight_kernel");
   return 0;
 }
 

@@ -641,3 +641,36 @@ class VectorQuantizeFn(torch.autograd.Function):
         bwd = ops.vq_bwd_deterministic if deterministic() else ops.vq_bwd
         gz, gE = bwd(z, E, idx, g_out, g_loss, residual, beta, use_norm)
         return gz, gE, None, None, None, None
+
+
+class EMAVectorQuantizeFn(torch.autograd.Function):
+    """EMAVectorQuantizer's lookup: the forward of VectorQuantizeFn with the EMA loss and, with `stats`, the flat per-code
+    statistics (non-differentiable).  E must be the codebook as it is at this forward and must not change before backward
+    (EMAVectorQuantizer passes a copy when an update follows).  The codebook gets no gradient."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, z, E, depth, beta, residual, use_norm, stats):
+        out, loss, idx, buf = ops.vq_fwd_ema(z, E, depth, beta, use_norm, stats, deterministic())
+        ctx.save_for_backward(z, E, idx)
+        ctx.cfg = (beta, residual, use_norm)
+        if buf is None:
+            ctx.mark_non_differentiable(idx)
+            return out, loss, idx
+        ctx.mark_non_differentiable(idx, buf)
+        return out, loss, idx, buf
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g_out, g_loss, _g_idx, _g_stats=None):
+        z, E, idx = ctx.saved_tensors
+        beta, residual, use_norm = ctx.cfg
+        if residual:
+            # the residual is built from z.detach() (quantizers.py:43): only the straight-through value reaches z
+            gz = g_out
+        else:
+            # d(beta * mean((sg(q) - norm(z))^2))/dz is exactly vq_bwd's gz (its codebook term only ever reached E);
+            # gz does not depend on how vq_bwd sums its codebook gradient, which is discarded here
+            gz, _ = ops.vq_bwd(z, E, idx, None if g_out is None else g_out.contiguous(),
+                               None if g_loss is None else g_loss.contiguous(), False, beta, use_norm)
+        return gz, None, None, None, None, None, None

@@ -328,6 +328,38 @@ def vq_bwd_deterministic(z: Tensor, E: Tensor, idx: Tensor, g_out: Optional[Tens
     return gz, gE
 
 
+def vq_fwd_ema(z: Tensor, E: Tensor, depth: int, beta: float, use_norm: bool = True, stats: bool = True,
+               deterministic: bool = False) -> Tuple[Tensor, Tensor, Tensor, Optional[Tensor]]:
+    """EMA-codebook lookup: (out, loss, idx) as vq_fwd (the loss without its codebook term) and, with stats, one flat fp32
+    buffer [K * (D + 1)]: the per-code sums s [K, D] followed by the counts n [K] -- the one tensor the replicas all-reduce.
+    deterministic: s summed in a fixed order."""
+    _req(z, "z"); _req(E, "embedding.weight")
+    K, D = E.shape
+    M = z.numel() // D
+    L = _lib.lib()
+    ws_bytes = L.b200vq_vq_fwd_ema_workspace_bytes(M, K, D, depth, int(deterministic))
+    ws = torch.empty(max(ws_bytes, 1), device=z.device, dtype=torch.uint8)
+    out = torch.empty_like(z)
+    idx = torch.empty(M, depth, device=z.device, dtype=torch.int64)
+    loss = torch.empty((), device=z.device, dtype=torch.float32)
+    buf = torch.empty(K * (D + 1), device=z.device, dtype=torch.float32) if stats else None
+    sums, counts = (buf[:K * D], buf[K * D:]) if stats else (None, None)
+    _lib.check(L.b200vq_vq_fwd_ema(_p(z), _p(E), _p(out), _p(idx), _p(loss), _p(counts), _p(sums), M, K, D, depth, float(beta),
+                                   int(use_norm), int(deterministic), _p(ws), ws_bytes, _stream()), "vq_fwd_ema")
+    return out, loss, idx, buf
+
+
+def vq_ema_update(stats: Tensor, cluster_size: Tensor, embed_avg: Tensor, weight: Tensor, decay: float, eps: float) -> None:
+    """in place: the EMA update of cluster_size [K], embed_avg [K, D] and weight [K, D] from vq_fwd_ema's flat statistics"""
+    _req(stats, "stats"); _req(cluster_size, "cluster_size"); _req(embed_avg, "embed_avg"); _req(weight, "embedding.weight")
+    K, D = weight.shape
+    if stats.numel() != K * (D + 1) or cluster_size.numel() != K or embed_avg.shape != weight.shape:
+        raise RuntimeError(f"b200vq: vq_ema_update shapes: stats {tuple(stats.shape)}, cluster_size {tuple(cluster_size.shape)}, "
+                           f"embed_avg {tuple(embed_avg.shape)}, weight {tuple(weight.shape)}")
+    _lib.check(_lib.lib().b200vq_vq_ema_update(_p(stats[K * D:]), _p(stats), _p(cluster_size), _p(embed_avg), _p(weight), K, D,
+                                               float(decay), float(eps), _stream()), "vq_ema_update")
+
+
 def vq_embed(E: Tensor, codes: Tensor, depth: int, use_norm: bool = True) -> Tensor:
     _req(E, "embedding.weight"); _req(codes, "codes", torch.int64)
     K, D = E.shape

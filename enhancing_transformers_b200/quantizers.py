@@ -74,6 +74,70 @@ class VectorQuantizer(BaseQuantizer):
                             bool(self.use_norm)).view(*lead, self.embed_dim)
 
 
+class EMAVectorQuantizer(VectorQuantizer):
+    """VectorQuantizer whose codebook is trained by exponential moving averages instead of gradients (van den Oord et al.
+    2017, appendix A.1, in the form of Taming Transformers' ``EMAVectorQuantizer``; RQ-VAE trains its shared codebook the
+    same way).  Same constructor plus ``decay`` and ``eps``, same lookup, codes and straight-through value; the loss is
+    ``beta * mean((sg(q) - norm(z))^2)`` (averaged over the depths in residual mode) without a codebook term, and
+    ``embedding.weight`` is frozen (``requires_grad = False``).
+
+    Every forward in training mode (``self.training``; grad mode does not matter) gathers, over all tokens and depths, the
+    count ``n_k`` and the sum ``s_k`` of the vectors the lookup compared per code, sums them over ``process_group`` (default:
+    WORLD) when torch.distributed runs with more than one rank -- one all-reduce of one flat fp32 buffer -- and then updates,
+    on the device::
+
+        cluster_size <- decay * cluster_size + (1 - decay) * n
+        embed_avg    <- decay * embed_avg    + (1 - decay) * s
+        weight_k      = embed_avg_k / ((cluster_size_k + eps) / (N + K * eps) * N),   N = sum_k cluster_size_k
+
+    The backward uses the codebook the forward looked up in.  Eval mode: the same lookup and loss, no update.  The buffers
+    ``cluster_size`` and ``embed_avg`` join VectorQuantizer's state-dict keys; a state dict without them (a gradient-trained
+    checkpoint) re-seeds them from the loaded weight as the constructor does."""
+
+    def __init__(self, embed_dim: int, n_embed: int, beta: float = 0.25, use_norm: bool = True,
+                 use_residual: bool = False, num_quantizers: Optional[int] = None, decay: float = 0.99, eps: float = 1e-5,
+                 **kwargs) -> None:
+        super().__init__(embed_dim, n_embed, beta, use_norm, use_residual, num_quantizers, **kwargs)
+        self.decay = decay
+        self.eps = eps
+        self.embedding.weight.requires_grad_(False)
+        self.register_buffer("cluster_size", torch.zeros(n_embed))
+        self.register_buffer("embed_avg", self.embedding.weight.detach().clone())
+        self.process_group = None
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs)
+        w = state_dict.get(prefix + "embedding.weight")
+        if w is None or tuple(w.shape) != tuple(self.embed_avg.shape):
+            return
+        with torch.no_grad():          # otherwise the first update would overwrite the loaded codebook
+            if prefix + "embed_avg" not in state_dict:
+                self.embed_avg.copy_(w)
+            if prefix + "cluster_size" not in state_dict:
+                self.cluster_size.zero_()
+
+    def forward(self, z: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        zc = z.contiguous()
+        weight = self.embedding.weight
+        update = self.training
+        # the update rewrites the weight in place, which autograd's version counter does not see: the backward gets a copy
+        E = weight.detach().clone() if update and torch.is_grad_enabled() else weight.detach()
+        res = Fn.EMAVectorQuantizeFn.apply(zc.view(-1, self.embed_dim), E, self.depth, float(self.beta), bool(self.use_residual),
+                                           bool(self.use_norm), update)
+        out, loss, idx = res[:3]
+        if update:
+            self._update(res[3])
+        out = out.view_as(zc)
+        idx = idx.view(*z.shape[:-1], self.depth) if self.use_residual else idx.view(*z.shape[:-1])
+        return out, loss, idx
+
+    def _update(self, stats: torch.Tensor) -> None:
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size(self.process_group) > 1:
+            dist.all_reduce(stats, op=dist.ReduceOp.SUM, group=self.process_group)
+        ops.vq_ema_update(stats, self.cluster_size, self.embed_avg, self.embedding.weight.data, self.decay, self.eps)
+
+
 class GumbelQuantizer(BaseQuantizer):
     """Drop-in for the reference's ``GumbelQuantizer`` (quantizers.py:95-126; used by ``ViTVQGumbel``, vitvqgan.py:147-176).
 

@@ -148,6 +148,21 @@ int b200vq_vq_bwd_deterministic(const float* z, const float* E, const long long*
 /* decode_codes (vitvqgan.py:81-86): out[m] = sum_t norm(E[codes[m,t]]) */
 int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
                     void* stream);
+/* EMA codebook (EMAVectorQuantizer; van den Oord et al. 2017 appendix A.1 as in Taming Transformers' EMAVectorQuantizer).
+ * vq_fwd_ema: the lookup of b200vq_vq_fwd (same out and idx, bit for bit) with the EMA loss beta * mean((q - x)^2), averaged
+ *   over the depths -- no codebook term.  counts [K] and sums [K,D] (both NULL: no statistics, e.g. in eval mode) are
+ *   overwritten with n_k = #{(m,t) : idx[m,t] = k} (exact integers in fp32) and s_k = sum of the vectors the lookup compared
+ *   for those entries (norm(residual_t[m]), or the raw residual when use_norm == 0).  deterministic == 0: s is summed with
+ *   float atomics (per-CTA shared-memory tables, then one global atomic per CTA, code and column); != 0: s is summed in
+ *   the fixed order of b200vq_vq_bwd_deterministic, the same bits on every run.  M * depth < 2^24; workspace from the query.
+ * vq_ema_update: in place, with no host synchronisation:
+ *   cluster_size = decay * cluster_size + (1 - decay) * counts;  embed_avg = decay * embed_avg + (1 - decay) * sums;
+ *   N = sum_k cluster_size_k (fixed order);  weight_k = embed_avg_k / ((cluster_size_k + eps) / (N + K * eps) * N). */
+size_t b200vq_vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int deterministic);
+int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, long long* idx, float* loss, float* counts, float* sums, int M, int K,
+                      int D, int depth, float beta, int use_norm, int deterministic, void* workspace, size_t ws_bytes, void* stream);
+int b200vq_vq_ema_update(const float* counts, const float* sums, float* cluster_size, float* embed_avg, float* weight, int K, int D,
+                         float decay, float eps, void* stream);
 
 /* ---- re-layout / reductions ------------------------------------------------------------------------*/
 /* [B,C,H,W] -> [B*(H/ph)*(W/pw), C*ph*pw], patch vector ordered (c,row,col) (layers.py:157-171); pw % 4 == 0 */
