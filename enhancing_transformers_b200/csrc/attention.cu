@@ -6,16 +6,11 @@
 // kernels of the fp16 data path; attention_exact.cu: mma.sync tf32 / 3xTF32 kernels and the
 // stage-2 mask); backward recomputes them from the saved log-sum-exp and needs
 // delta = rowsum(dO * O), computed below.
+#include "../../include/b200vq.h"
+#include "attention.cuh"
 #include "common.cuh"
 
 namespace b200 {
-
-int attention_forward_tc(const float*, void*, int, float*, int, int, int, int, float, int, int, cudaStream_t);
-int attention_backward_tc(const float*, const float*, const float*, const float*, void*, int, const float*, int, int, int, int,
-                          float, int, int, cudaStream_t);
-int attention_exact_forward(const float*, float*, float*, int, int, int, int, float, int, cudaStream_t);
-int attention_exact_backward(const float*, const float*, const float*, const float*, float*, float*, int, int, int, int, float, int,
-                             cudaStream_t);
 
 // delta[b,h,n] = sum_d dO[b,n,h,d] * O[b,n,h,d].  HBM-bound: one float4 of O and dO per thread, dh/4 adjacent
 // lanes per (row, head) reduced with shuffles, so a warp streams 512 contiguous bytes of each tensor.
@@ -53,13 +48,6 @@ attn_delta_kernel(const void* __restrict__ o, const void* __restrict__ dout, flo
   }
 }
 
-int attention_forward(const float* qkv, void* out, int out_half, float* lse, int B, int N, int heads, int dh, float scale,
-                      int round_out, cudaStream_t stream) {
-  B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
-  B200_CHECK_ARG(dh == 64 || dh == 32, "attention: dim_head must be 32 or 64 (got %d)", dh);
-  return attention_forward_tc(qkv, out, out_half, lse, B, N, heads, dh, scale, round_out, -1, stream);
-}
-
 int attention_delta(const void* out, int out_half, const void* dout, int dout_half, float* delta, int B, int N, int heads, int dh,
                     cudaStream_t stream) {
   const long long groups = (long long)B * N * heads;
@@ -85,9 +73,22 @@ int attention_delta(const void* out, int out_half, const void* dout, int dout_ha
   return 0;
 }
 
-int attention_backward(const float* qkv, const void* out, int out_half, const float* lse, const float* dout, void* dqkv,
-                       int dqkv_half, const float* dqkv_scale, float* delta, int B, int N, int heads, int dh, float scale,
-                       int round_out, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" int b200vq_attention_fwd(const float* qkv, void* out, int out_half, float* lse, int B, int N, int heads, int dh,
+                                    float scale, int round_out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
+  B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
+  B200_CHECK_ARG(dh == 64 || dh == 32, "attention: dim_head must be 32 or 64 (got %d)", dh);
+  return attention_forward_tc(qkv, out, out_half, lse, B, N, heads, dh, scale, round_out, -1, stream);
+}
+
+extern "C" int b200vq_attention_bwd(const float* qkv, const void* out, int out_half, const float* lse, const float* dout, void* dqkv,
+                                    int dqkv_half, const float* dqkv_scale, float* delta, int B, int N, int heads, int dh,
+                                    float scale, int round_out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
   B200_CHECK_ARG(dh == 64 || dh == 32, "attention: dim_head must be 32 or 64 (got %d)", dh);
   int rc = attention_delta(out, out_half, dout, 0, delta, B, N, heads, dh, stream);
@@ -99,8 +100,9 @@ int attention_backward(const float* qkv, const void* out, int out_half, const fl
 // condition prefix) see each other fully -- query q attends to key k iff k <= max(q, cond_len - 1).  Same packed qkv layout
 // as the stage-1 core (the reference's (T, B*nh, hs) views are that layout transposed).  exact != 0: 3xTF32 mma.sync kernels
 // (precision="parity"); otherwise the single-pass tf32 kernels with the same mask.
-int attention_causal_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale, int cond_len,
-                             int exact, int round_out, cudaStream_t stream) {
+extern "C" int b200vq_attention_causal_fwd(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
+                                           int cond_len, int exact, int round_out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
   B200_CHECK_ARG(dh == 64 || dh == 32, "attention: head size must be 32 or 64 (got %d)", dh);
   B200_CHECK_ARG(cond_len >= 0 && cond_len <= N, "attention: cond_len %d outside [0, %d]", cond_len, N);
@@ -108,9 +110,10 @@ int attention_causal_forward(const float* qkv, float* out, float* lse, int B, in
   return attention_forward_tc(qkv, out, 0, lse, B, N, heads, dh, scale, round_out, cond_len, stream);
 }
 
-int attention_causal_backward(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv, float* delta,
-                              int B, int N, int heads, int dh, float scale, int cond_len, int exact, int round_out,
-                              cudaStream_t stream) {
+extern "C" int b200vq_attention_causal_bwd(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv,
+                                           float* delta, int B, int N, int heads, int dh, float scale, int cond_len, int exact,
+                                           int round_out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
   B200_CHECK_ARG(dh == 64 || dh == 32, "attention: head size must be 32 or 64 (got %d)", dh);
   B200_CHECK_ARG(cond_len >= 0 && cond_len <= N, "attention: cond_len %d outside [0, %d]", cond_len, N);
@@ -119,5 +122,3 @@ int attention_causal_backward(const float* qkv, const float* out, const float* l
   if (rc) return rc;
   return attention_backward_tc(qkv, dout, lse, delta, dqkv, 0, nullptr, B, N, heads, dh, scale, round_out, cond_len, stream);
 }
-
-}  // namespace b200

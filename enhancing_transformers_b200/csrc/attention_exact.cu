@@ -9,6 +9,8 @@
 // OUT16 selects fp16 storage of the outputs (O, dq/dk/dv).  The fp16 data path runs on wgmma in attention_f16.cu.
 // Backward is split in two kernels so that no atomics are needed: one CTA per key tile (dK, dV) and one per
 // query tile (dQ).
+#include "../../include/b200vq.h"
+#include "attention.cuh"
 #include "common.cuh"
 
 namespace b200 {
@@ -488,10 +490,6 @@ static int bwd_launch(const void* qkv, const void* dout, const float* lse, const
   return 0;
 }
 
-// delta = rowsum(dO * O) through the shared helper of attention.cu
-int attention_delta(const void* out, int out_half, const void* dout, int dout_half, float* delta, int B, int N, int heads, int dh,
-                    cudaStream_t stream);
-
 static int check_problem(const void* qkv, int B, int N, int heads, int dh, int cond_len) {
   B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
   B200_CHECK_ARG(dh == 64 || dh == 32, "attention: dim_head must be 32 or 64 (got %d)", dh);
@@ -501,7 +499,6 @@ static int check_problem(const void* qkv, int B, int N, int heads, int dh, int c
   return 0;
 }
 
-// cond_len < 0: no mask (stage 1).  cond_len >= 0: the stage-2 mask, causal with a fully visible prefix of cond_len tokens.
 int attention_exact_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
                             int cond_len, cudaStream_t stream) {
   if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
@@ -518,7 +515,6 @@ int attention_exact_backward(const float* qkv, const float* out, const float* ls
   return bwd_launch<32, 3, 0>(qkv, dout, lse, delta, dqkv, nullptr, B, N, heads, scale, cond_len, 0, stream);
 }
 
-// tf32 core: fp32 q/k/v (tf32-rounded by the GEMM that wrote them); O in fp32 (optionally tf32-rounded) or fp16
 int attention_forward_tc(const float* qkv, void* out, int out_half, float* lse, int B, int N, int heads, int dh, float scale,
                          int round_out, int cond_len, cudaStream_t stream) {
   if (int rc = check_problem(qkv, B, N, heads, dh, cond_len)) return rc;
@@ -528,7 +524,6 @@ int attention_forward_tc(const float* qkv, void* out, int out_half, float* lse, 
                   : fwd_launch<32, 1, 0>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
 }
 
-// delta must already hold rowsum(dO * O).  dqkv fp32 (optionally tf32-rounded) or, with out_half, fp16(dqkv * out_scale[0]).
 int attention_backward_tc(const float* qkv, const float* dout, const float* lse, const float* delta, void* dqkv, int out_half,
                           const float* out_scale, int B, int N, int heads, int dh, float scale, int round_out, int cond_len,
                           cudaStream_t stream) {
@@ -541,3 +536,15 @@ int attention_backward_tc(const float* qkv, const float* dout, const float* lse,
 }
 
 }  // namespace b200
+
+using namespace b200;
+
+extern "C" int b200vq_attention_exact_fwd(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
+                                          void* streamv) {
+  return attention_exact_forward(qkv, out, lse, B, N, heads, dh, scale, -1, static_cast<cudaStream_t>(streamv));
+}
+
+extern "C" int b200vq_attention_exact_bwd(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv,
+                                          float* delta, int B, int N, int heads, int dh, float scale, void* streamv) {
+  return attention_exact_backward(qkv, out, lse, dout, dqkv, delta, B, N, heads, dh, scale, -1, static_cast<cudaStream_t>(streamv));
+}

@@ -17,6 +17,8 @@
 //                S^T = K Q^T, dP^T = V dO^T, dV += P^T dO, dK += dS^T Q
 //   query side   128 queries per CTA, Q and dO resident; K / V tiles: S = Q K^T, dP = dO V^T, dQ += dS K
 // Backward is two kernels so that no atomics are needed: a run is bit-reproducible.
+#include "../../include/b200vq.h"
+#include "attention.cuh"
 #include "common.cuh"
 
 namespace b200 {
@@ -409,9 +411,13 @@ attn_f16_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_
   }
 }
 
+}  // namespace b200
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+using namespace b200;
+
 // one image's rows of a packed fp16 [B*N, cols] matrix as {cols, N, B}; 64 x 64 boxes (one head, 64 rows)
 static int rows_map(CUtensorMap* m, const void* p, int B, int N, long long cols) {
   const unsigned long long dims[3] = {(unsigned long long)cols, (unsigned long long)N, (unsigned long long)B};
@@ -434,7 +440,9 @@ static int check_problem(const void* qkv, const void* out, int B, int N, int hea
 }
 
 // q/k/v fp16 as the to_qkv GEMM stores them, O fp16, LSE fp32 [B, heads, N]
-int attention_f16_forward(const void* qkv, void* out, float* lse, int B, int N, int heads, int dh, float scale, cudaStream_t stream) {
+extern "C" int b200vq_attention_f16_fwd(const void* qkv, void* out, float* lse, int B, int N, int heads, int dh, float scale,
+                                        void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = check_problem(qkv, out, B, N, heads, dh)) return rc;
   CUtensorMap tm;
   if (int rc = rows_map(&tm, qkv, B, N, 3ll * heads * kDh)) return rc;
@@ -445,14 +453,11 @@ int attention_f16_forward(const void* qkv, void* out, float* lse, int B, int N, 
   return 0;
 }
 
-// delta = rowsum(dO * O) through the shared helper of attention.cu
-int attention_delta(const void* out, int out_half, const void* dout, int dout_half, float* delta, int B, int N, int heads, int dh,
-                    cudaStream_t stream);
-
 // dO fp16 carrying the power-of-two gradient scale S of the backward segment (functional.py); delta, dS and the stored
 // fp16 dq / dk / dv carry S too -- everything is linear in dO, nothing is rescaled here.
-int attention_f16_backward(const void* qkv, const void* out, const float* lse, const void* dout, void* dqkv, float* delta, int B, int N,
-                           int heads, int dh, float scale, cudaStream_t stream) {
+extern "C" int b200vq_attention_f16_bwd(const void* qkv, const void* out, const float* lse, const void* dout, void* dqkv, float* delta,
+                                        int B, int N, int heads, int dh, float scale, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = check_problem(qkv, out, B, N, heads, dh)) return rc;
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dout) & 15) == 0 && (reinterpret_cast<uintptr_t>(dqkv) & 15) == 0,
                  "attention: dout and dqkv must be 16-byte aligned");
@@ -470,5 +475,3 @@ int attention_f16_backward(const void* qkv, const void* out, const float* lse, c
   B200_LAUNCH_OK("attn_f16_bwd_dq_kernel");
   return 0;
 }
-
-}  // namespace b200

@@ -31,6 +31,7 @@
 // Warp roles (288 threads): warps 0..7 consume, warp 8 is the TMA producer.  fp16: warpgroup w (warps 4w..4w+3) owns
 // rows 64w .. 64w+63 of the 128 x 256 tile (warp 4w+i: rows 64w+16i .. +15); tf32: warp w owns rows 32*(w%4) .. +31
 // and half of the BN columns.
+#include "../../include/b200vq.h"
 #include "common.cuh"
 
 #include <mutex>
@@ -656,29 +657,35 @@ static int gemm_launch(int kind, const void* A, long long lda, int a_major, cons
   return bn == 64 ? dispatch_major<0, 64>(a_major, b_major, 0, tm, p, stream) : dispatch_major<0, 128>(a_major, b_major, 0, tm, p, stream);
 }
 
-int gemm_tf32(const float* A, long long lda, int a_major, const float* B, long long ldb, int b_major, float* C,
-              long long ldc, int M, int N, int K, int splits, long long c_split_stride, const float* bias,
-              const float* res, long long ldres, int res_row_mod, const float* aux, long long ldaux,
-              float* colsum_part, int act, int round_out, int cta_group, int bn, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" int b200vq_gemm_tf32(const float* A, long long lda, int a_major, const float* B, long long ldb, int b_major, float* C,
+                                long long ldc, int M, int N, int K, int splits, long long c_split_stride, const float* bias,
+                                const float* res, long long ldres, int res_row_mod, const float* aux, long long ldaux,
+                                float* colsum_part, int act, int round_out, int cta_group, int bn, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   return gemm_launch(0, A, lda, a_major, B, ldb, b_major, C, ldc, 0, M, N, K, splits, c_split_stride, bias, res, ldres, res_row_mod,
                      aux, ldaux, colsum_part, act, round_out, nullptr, nullptr, nullptr, cta_group, bn, stream);
 }
 
-int gemm_3xtf32(const float* A, const float* A_lo, long long lda, int a_major, const float* B, const float* B_lo, long long ldb,
-                int b_major, float* C, long long ldc, int M, int N, int K, int splits, long long c_split_stride,
-                const float* bias, const float* res, long long ldres, int res_row_mod, const float* aux, long long ldaux,
-                float* colsum_part, int act, int cta_group, int bn, cudaStream_t stream) {
+extern "C" int b200vq_gemm_3xtf32(const float* A, const float* A_lo, long long lda, int a_major, const float* B, const float* B_lo,
+                                  long long ldb, int b_major, float* C, long long ldc, int M, int N, int K, int splits,
+                                  long long c_split_stride, const float* bias, const float* res, long long ldres, int res_row_mod,
+                                  const float* aux, long long ldaux, float* colsum_part, int act, int cta_group, int bn, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(A_lo && B_lo, "gemm_3xtf32: A_lo and B_lo are required");
   return gemm_launch(0, A, lda, a_major, B, ldb, b_major, C, ldc, 0, M, N, K, splits, c_split_stride, bias, res, ldres, res_row_mod,
                      aux, ldaux, colsum_part, act, 0, nullptr, A_lo, B_lo, cta_group, bn, stream);
 }
 
-int gemm_f16(const void* A, long long lda, int a_major, const void* B, long long ldb, int b_major, void* C, long long ldc,
-             int out_half, int M, int N, int K, int splits, long long c_split_stride, const float* bias, const float* res,
-             long long ldres, int res_row_mod, const void* aux, long long ldaux, float* colsum_part, int act, int round_out,
-             const float* alpha_ptr, int cta_group, int bn, cudaStream_t stream) {
+extern "C" int b200vq_gemm_f16(const void* A, long long lda, int a_major, const void* B, long long ldb, int b_major, void* C,
+                               long long ldc, int out_half, int M, int N, int K, int splits, long long c_split_stride,
+                               const float* bias, const float* res, long long ldres, int res_row_mod, const void* aux,
+                               long long ldaux, float* colsum_part, int act, int round_out, const float* alpha_ptr, int cta_group,
+                               int bn, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   return gemm_launch(1, A, lda, a_major, B, ldb, b_major, C, ldc, out_half, M, N, K, splits, c_split_stride, bias, res, ldres,
                      res_row_mod, aux, ldaux, colsum_part, act, round_out, alpha_ptr, nullptr, nullptr, cta_group, bn, stream);
 }
-
-}  // namespace b200

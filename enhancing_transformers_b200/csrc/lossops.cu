@@ -6,6 +6,7 @@
 // Both are HBM-bound streams: float4 grid-stride loops sized to the SM count; the FIR reads each input pixel from L1/L2
 // for its <= 16 taps (4 x 4 blur kernels in every shipped discriminator).  The JIT-compiled extensions of the
 // reference (torch.utils.cpp_extension.load at import time) are not needed once loss_ops.py is installed.
+#include "../../include/b200vq.h"
 #include "common.cuh"
 
 namespace b200 {
@@ -71,8 +72,13 @@ static inline int lo_grid(long long work, int threads) {
   return (int)(blocks < 1 ? 1 : blocks);
 }
 
-int bias_act(const float* x, const float* b, const float* ref, float* out, long long n, int step_b, int size_b, int act, int grad,
-             float alpha, float scale, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" int b200vq_bias_act(const float* x, const float* b, const float* ref, float* out, long long n, int step_b, int size_b,
+                               int act, int grad, float alpha, float scale, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n > 0, "bias_act: empty input");
   B200_CHECK_ARG(act == 1 || act == 3, "bias_act: act must be 1 (linear) or 3 (leaky ReLU), got %d", act);
   B200_CHECK_ARG(grad >= 0 && grad <= 2, "bias_act: grad must be 0, 1 or 2");
@@ -84,8 +90,10 @@ int bias_act(const float* x, const float* b, const float* ref, float* out, long 
   return 0;
 }
 
-int upfirdn2d(const float* in, const float* kern, float* out, long long planes, int in_h, int in_w, int kh, int kw, int up_x, int up_y,
-              int down_x, int down_y, int pad_x0, int pad_x1, int pad_y0, int pad_y1, cudaStream_t stream) {
+extern "C" int b200vq_upfirdn2d(const float* in, const float* kern, float* out, long long planes, int in_h, int in_w, int kh, int kw,
+                                int up_x, int up_y, int down_x, int down_y, int pad_x0, int pad_x1, int pad_y0, int pad_y1,
+                                void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(planes > 0 && in_h > 0 && in_w > 0 && kh > 0 && kw > 0 && kh * kw <= 1024, "upfirdn2d: bad sizes");
   B200_CHECK_ARG(up_x > 0 && up_y > 0 && down_x > 0 && down_y > 0, "upfirdn2d: up/down factors must be positive");
   const int out_h = (in_h * up_y + pad_y0 + pad_y1 - kh + down_y) / down_y;
@@ -96,5 +104,3 @@ int upfirdn2d(const float* in, const float* kern, float* out, long long planes, 
   B200_LAUNCH_OK("upfirdn2d_kernel");
   return 0;
 }
-
-}  // namespace b200

@@ -2,6 +2,7 @@
 // (reference layers.py:85-92,143,150), patch <-> image re-layout for the kernel==stride
 // convolutions (layers.py:168-171,202-205), column sums (bias gradients), split-K reduction
 // and tf32 rounding of GEMM operands.  All are coalesced float4 streams sized to the SM count.
+#include "../../include/b200vq.h"
 #include "common.cuh"
 
 namespace b200 {
@@ -454,6 +455,10 @@ static inline int stream_grid(long long work_items, int threads) {
   return (int)blocks;
 }
 
+}  // namespace b200
+
+using namespace b200;
+
 template <int NV>
 static void ln_fwd_launch(const float* x, const float* g, const float* b, float* y, __half* y16, float* mean, float* rstd, int M,
                           int D, int round_out, cudaStream_t s) {
@@ -461,8 +466,9 @@ static void ln_fwd_launch(const float* x, const float* g, const float* b, float*
   ln_fwd_kernel<NV><<<blocks, 256, 0, s>>>(x, g, b, y, y16, mean, rstd, M, D, round_out);
 }
 
-int layernorm_forward(const float* x, const float* gamma, const float* beta, float* y, void* y16v, float* mean, float* rstd,
-                      int M, int D, int round_out, cudaStream_t stream) {
+extern "C" int b200vq_layernorm_fwd(const float* x, const float* gamma, const float* beta, float* y, void* y16v, float* mean,
+                                    float* rstd, int M, int D, int round_out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(M > 0 && D > 0 && D % 4 == 0 && D <= 2048, "layernorm: need D %% 4 == 0 and D <= 2048 (D=%d)", D);
   B200_CHECK_ARG(y || y16v, "layernorm: no output buffer");
   __half* y16 = static_cast<__half*>(y16v);
@@ -477,8 +483,8 @@ int layernorm_forward(const float* x, const float* gamma, const float* beta, flo
   return 0;
 }
 
-int layernorm_bwd_blocks() { return num_sms() * 2; }
-size_t layernorm_bwd_workspace_bytes(int D) { return (size_t)layernorm_bwd_blocks() * 3 * D * sizeof(float); }
+static int layernorm_bwd_blocks() { return num_sms() * 2; }
+extern "C" size_t b200vq_layernorm_bwd_workspace_bytes(int D) { return (size_t)layernorm_bwd_blocks() * 3 * D * sizeof(float); }
 
 template <int NV, int NACC>
 static int ln_bwd_launch(const void* dy, int dy_half, const float* dy_scale, const float* x, const float* mean, const float* rstd, const float* gamma,
@@ -504,12 +510,14 @@ static int ln_bwd_dispatch(const void* dy, int dy_half, const float* dy_scale, c
   return ln_bwd_launch<16, NACC>(dy, dy_half, dy_scale, x, mean, rstd, gamma, dres, dx, dx16, scale_ptr, part, M, D, round_out, blocks, s);
 }
 
-int layernorm_backward(const void* dy, int dy_half, const float* dy_scale, const float* x, const float* mean, const float* rstd, const float* gamma,
-                       const float* dres, float* dx, void* dx16v, const float* scale_ptr, float* dgamma, float* dbeta,
-                       float* dxsum, int M, int D, int round_out, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_layernorm_bwd(const void* dy, int dy_half, const float* dy_scale, const float* x, const float* mean,
+                                    const float* rstd, const float* gamma, const float* dres, float* dx, void* dx16v,
+                                    const float* scale_ptr, float* dgamma, float* dbeta, float* dxsum, int M, int D, int round_out,
+                                    void* workspace, size_t ws_bytes, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   __half* dx16 = static_cast<__half*>(dx16v);
   B200_CHECK_ARG(M > 0 && D > 0 && D % 4 == 0 && D <= 2048, "layernorm: need D %% 4 == 0 and D <= 2048 (D=%d)", D);
-  B200_CHECK_ARG(ws_bytes >= layernorm_bwd_workspace_bytes(D), "layernorm_backward: workspace too small");
+  B200_CHECK_ARG(ws_bytes >= b200vq_layernorm_bwd_workspace_bytes(D), "layernorm_backward: workspace too small");
   int blocks = layernorm_bwd_blocks();
   if (blocks > (M + 7) / 8) blocks = (M + 7) / 8;
   float* part = static_cast<float*>(workspace);
@@ -524,11 +532,13 @@ int layernorm_backward(const void* dy, int dy_half, const float* dy_scale, const
 }
 
 constexpr int kColsumMaxSplits = 64;
-size_t colsum_workspace_bytes(int N) { return (size_t)kColsumMaxSplits * N * sizeof(float); }
+extern "C" size_t b200vq_colsum_workspace_bytes(int N) { return (size_t)kColsumMaxSplits * N * sizeof(float); }
 
-int colsum(const float* X, long long ld, int M, int N, float* out, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_colsum(const float* X, long long ld, int M, int N, float* out, void* workspace, size_t ws_bytes,
+                             void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(M > 0 && N > 0 && N % 4 == 0 && ld % 4 == 0, "colsum: N and ld must be multiples of 4");
-  B200_CHECK_ARG(ws_bytes >= colsum_workspace_bytes(N), "colsum: workspace too small");
+  B200_CHECK_ARG(ws_bytes >= b200vq_colsum_workspace_bytes(N), "colsum: workspace too small");
   const int colblocks = (N / 4 + 31) / 32;
   int splits = (num_sms() * 8 + colblocks - 1) / colblocks;
   if (splits > kColsumMaxSplits) splits = kColsumMaxSplits;
@@ -542,29 +552,33 @@ int colsum(const float* X, long long ld, int M, int N, float* out, void* workspa
   return 0;
 }
 
-int splitk_reduce(const float* part, int splits, long long n, long long split_stride, const float* alpha_ptr, float* out,
-                  cudaStream_t stream) {
+extern "C" int b200vq_splitk_reduce(const float* part, int splits, long long n, long long split_stride, const float* alpha_ptr,
+                                    float* out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n % 4 == 0 && split_stride % 4 == 0, "splitk_reduce: sizes must be multiples of 4");
   splitk_reduce_kernel<<<stream_grid(n / 4, 256), 256, 0, stream>>>(part, splits, n / 4, split_stride / 4, alpha_ptr, out);
   B200_LAUNCH_OK("splitk_reduce_kernel");
   return 0;
 }
 
-int round_tf32_copy(const float* in, float* out, long long n, cudaStream_t stream) {
+extern "C" int b200vq_round_tf32(const float* in, float* out, long long n, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n % 4 == 0, "round_tf32: n %% 4");
   round_tf32_kernel<<<stream_grid(n / 4, 256), 256, 0, stream>>>(in, out, n / 4);
   B200_LAUNCH_OK("round_tf32_kernel");
   return 0;
 }
 
-int split_tf32_lo(const float* in, float* lo, long long n, cudaStream_t stream) {
+extern "C" int b200vq_split_tf32_lo(const float* in, float* lo, long long n, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n % 4 == 0, "split_tf32_lo: n %% 4");
   split_tf32_lo_kernel<<<stream_grid(n / 4, 256), 256, 0, stream>>>(in, lo, n / 4);
   B200_LAUNCH_OK("split_tf32_lo_kernel");
   return 0;
 }
 
-int to_half(const float* in, void* out, long long n, const float* scale_ptr, cudaStream_t stream) {
+extern "C" int b200vq_to_half(const float* in, void* out, long long n, const float* scale_ptr, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n % 4 == 0, "to_half: n %% 4");
   to_half_kernel<<<stream_grid(n / 4, 256), 256, 0, stream>>>(in, static_cast<__half*>(out), n / 4, scale_ptr);
   B200_LAUNCH_OK("to_half_kernel");
@@ -572,10 +586,12 @@ int to_half(const float* in, void* out, long long n, const float* scale_ptr, cud
 }
 
 constexpr int kAbsmaxBlocks = 1056;   // 132 SMs x 8
-size_t grad_scale_workspace_bytes() { return kAbsmaxBlocks * sizeof(unsigned); }
-int grad_scale(const float* g, long long n, int target_log2, float* scale2, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+extern "C" size_t b200vq_grad_scale_workspace_bytes(void) { return kAbsmaxBlocks * sizeof(unsigned); }
+extern "C" int b200vq_grad_scale(const float* g, long long n, int target_log2, float* scale2, void* workspace, size_t ws_bytes,
+                                 void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n > 0 && n % 4 == 0, "grad_scale: n %% 4");
-  B200_CHECK_ARG(ws_bytes >= grad_scale_workspace_bytes(), "grad_scale: workspace too small");
+  B200_CHECK_ARG(ws_bytes >= b200vq_grad_scale_workspace_bytes(), "grad_scale: workspace too small");
   B200_CHECK_ARG(target_log2 >= -14 && target_log2 <= 15, "grad_scale: target exponent outside the fp16 range");
   int blocks = stream_grid(n / 4, 256);
   if (blocks > kAbsmaxBlocks) blocks = kAbsmaxBlocks;
@@ -587,14 +603,17 @@ int grad_scale(const float* g, long long n, int target_log2, float* scale2, void
   return 0;
 }
 
-int add_rows_mod(const float* x, const float* table, float* out, long long M, int D, int R, cudaStream_t stream) {
+extern "C" int b200vq_add_rows_mod(const float* x, const float* table, float* out, long long M, int D, int R, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D % 4 == 0 && R > 0 && M > 0, "add_rows_mod: D %% 4 and R > 0 required");
   add_rows_mod_kernel<<<stream_grid(M * (D / 4), 256), 256, 0, stream>>>(x, table, out, M, D / 4, R);
   B200_LAUNCH_OK("add_rows_mod_kernel");
   return 0;
 }
 
-int patchify(const float* img, float* out, int B, int C, int H, int W, int ph, int pw, int round_out, cudaStream_t stream) {
+extern "C" int b200vq_patchify(const float* img, float* out, int B, int C, int H, int W, int ph, int pw, int round_out,
+                               void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(ph > 0 && pw > 0 && pw % 4 == 0 && H % ph == 0 && W % pw == 0,
                  "patchify: the patch must divide the image and its width must be a multiple of 4 (got %d x %d)", ph, pw);
   patchify_kernel<<<stream_grid((long long)B * C * H * W / 4, 256), 256, 0, stream>>>(img, out, B, C, H, W, ph, pw, round_out);
@@ -602,12 +621,12 @@ int patchify(const float* img, float* out, int B, int C, int H, int W, int ph, i
   return 0;
 }
 
-int unpatchify(const float* tok, const float* bias, float* img, int B, int C, int H, int W, int ph, int pw, cudaStream_t stream) {
+extern "C" int b200vq_unpatchify(const float* tok, const float* bias, float* img, int B, int C, int H, int W, int ph, int pw,
+                                 void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(ph > 0 && pw > 0 && pw % 4 == 0 && H % ph == 0 && W % pw == 0,
                  "unpatchify: the patch must divide the image and its width must be a multiple of 4 (got %d x %d)", ph, pw);
   unpatchify_kernel<<<stream_grid((long long)B * C * H * W / 4, 256), 256, 0, stream>>>(tok, bias, img, B, C, H, W, ph, pw);
   B200_LAUNCH_OK("unpatchify_kernel");
   return 0;
 }
-
-}  // namespace b200

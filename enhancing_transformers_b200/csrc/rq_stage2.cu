@@ -11,6 +11,7 @@
 // embedding rows equal the reference's bit for bit.  Their backward is linear: the raw gradient rows are summed by id
 // (float atomics, or scatter_det.cu's fixed-order sum on request) and one reverse channel scan over the [V, C] table
 // follows; no per-entry scan is materialised.
+#include "../../include/b200vq.h"
 #include "common.cuh"
 #include "scatter_det.cuh"
 
@@ -358,7 +359,11 @@ code_sum_embed_kernel(const long long* __restrict__ codes, long long ld, int n, 
   }
 }
 
+}  // namespace b200
+
 // ------------------------------------------------------------------------------------------------ host side
+using namespace b200;
+
 static int short_check(const void* a, const void* b, const void* c, long long nseq, int D, int heads, int hs, int cond,
                        const char* what) {
   B200_CHECK_ARG(a && b && c, "%s: null pointer argument", what);
@@ -385,8 +390,9 @@ static int short_warps(size_t warp_bytes) {
   return w < 1 ? 1 : (w > 8 ? 8 : w);
 }
 
-int short_attention_forward(const float* qkv, float* out, long long nseq, int D, int heads, int hs, int cond, float scale,
-                            cudaStream_t stream) {
+extern "C" int b200vq_short_attention_fwd(const float* qkv, float* out, long long nseq, int D, int heads, int hs, int cond,
+                                          float scale, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = short_check(qkv, out, out, nseq, D, heads, hs, cond, "short_attention_fwd")) return rc;
   const size_t wb = short_warp_floats(D, hs, 3) * sizeof(float);
   const int wpb = short_warps(wb);
@@ -397,8 +403,9 @@ int short_attention_forward(const float* qkv, float* out, long long nseq, int D,
   return 0;
 }
 
-int short_attention_backward(const float* qkv, const float* dout, float* dqkv, long long nseq, int D, int heads, int hs, int cond,
-                             float scale, cudaStream_t stream) {
+extern "C" int b200vq_short_attention_bwd(const float* qkv, const float* dout, float* dqkv, long long nseq, int D, int heads, int hs,
+                                          int cond, float scale, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = short_check(qkv, dout, dqkv, nseq, D, heads, hs, cond, "short_attention_bwd")) return rc;
   const size_t wb = short_warp_floats(D, hs, 4) * sizeof(float);
   const int wpb = short_warps(wb);
@@ -430,8 +437,10 @@ static int reverse_scan_rows(float* t, int V, int C, cudaStream_t stream) {
   return 0;
 }
 
-int rq_embed_forward(const long long* conds, const long long* codes, const float* Wc, const float* pos_c, const float* Wi,
-                     const float* pos_i, float* x, int B, int Tc, int T, int D, int C, int Vc, int Vi, cudaStream_t stream) {
+extern "C" int b200vq_rq_embed_fwd(const long long* conds, const long long* codes, const float* Wc, const float* pos_c,
+                                   const float* Wi, const float* pos_i, float* x, int B, int Tc, int T, int D, int C, int Vc, int Vi,
+                                   void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = embed_shape_ok(B, Tc, T, D, C, Vc, Vi, "rq_embed_fwd")) return rc;
   B200_CHECK_ARG(codes && Wi && pos_i && x && (Tc == 0 || (conds && Wc && pos_c)), "rq_embed_fwd: null pointer argument");
   rq_embed_fwd_kernel<<<rq_grid((long long)B * (Tc + T), 8), 256, 0, stream>>>(conds, codes, Wc, pos_c, Wi, pos_i, x, B, Tc, T, D, C,
@@ -442,8 +451,10 @@ int rq_embed_forward(const long long* conds, const long long* codes, const float
 
 // gWc / gWi zero-filled, then the cond rows and the code rows scattered with atomics; gpos = column sums over the batch;
 // gWi reverse-scanned
-int rq_embed_backward(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c, float* gWi,
-                      float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi, cudaStream_t stream) {
+extern "C" int b200vq_rq_embed_bwd(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                   float* gWi, float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi,
+                                   void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = embed_shape_ok(B, Tc, T, D, C, Vc, Vi, "rq_embed_bwd")) return rc;
   B200_CHECK_ARG(codes && g && gWi && gpos_i && (Tc == 0 || (conds && gWc && gpos_c)), "rq_embed_bwd: null pointer argument");
   const int Tt = Tc + T;
@@ -466,21 +477,22 @@ int rq_embed_backward(const long long* conds, const long long* codes, const floa
 
 static size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
 
-size_t rq_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int T, int D, int C, int Vc, int Vi) {
+extern "C" size_t b200vq_rq_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int T, int D, int C, int Vc, int Vi) {
   if (B <= 0 || Tc < 0 || T <= 0 || C <= 0 || D < 1 || Vi <= 0) return 0;
   const size_t wc = (Tc > 0 && Vc > 0) ? scatter_det_workspace_bytes((long long)B * Tc, Vc, C, kScatterRunToken) : 0;
   const size_t wi = scatter_det_workspace_bytes((long long)B * T, Vi, C, kScatterRunToken);
   return align256((size_t)B * T * sizeof(long long)) + (wc > wi ? wc : wi);
 }
 
-int rq_embed_backward_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
-                                    float* gWi, float* gpos_i, int B, int Tc, int T, int D, int C, int Vc, int Vi, void* workspace,
-                                    size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_rq_embed_bwd_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc,
+                                                 float* gpos_c, float* gWi, float* gpos_i, int B, int Tc, int T, int D, int C, int Vc,
+                                                 int Vi, void* workspace, size_t ws_bytes, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = embed_shape_ok(B, Tc, T, D, C, Vc, Vi, "rq_embed_bwd_deterministic")) return rc;
   B200_CHECK_ARG(codes && g && gWi && gpos_i && workspace && (Tc == 0 || (conds && gWc && gpos_c)),
                  "rq_embed_bwd_deterministic: null pointer argument");
   B200_CHECK_ARG((long long)B * (Tc + T) <= (1LL << 30), "rq_embed_bwd_deterministic: too many tokens");
-  B200_CHECK_ARG(ws_bytes >= rq_embed_bwd_deterministic_workspace_bytes(B, Tc, T, D, C, Vc, Vi),
+  B200_CHECK_ARG(ws_bytes >= b200vq_rq_embed_bwd_deterministic_workspace_bytes(B, Tc, T, D, C, Vc, Vi),
                  "rq_embed_bwd_deterministic: workspace too small");
   const long long Tt = Tc + T;
   long long* ids = static_cast<long long*>(workspace);
@@ -507,8 +519,9 @@ static int depth_shape_ok(long long nseq, int D, int C, int Vi, const char* what
   return 0;
 }
 
-int rq_depth_input_forward(const float* h, const long long* codes, const float* Wi, const float* pos_d, float* v, long long nseq, int D,
-                           int C, int Vi, cudaStream_t stream) {
+extern "C" int b200vq_rq_depth_input_fwd(const float* h, const long long* codes, const float* Wi, const float* pos_d, float* v,
+                                         long long nseq, int D, int C, int Vi, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = depth_shape_ok(nseq, D, C, Vi, "rq_depth_input_fwd")) return rc;
   B200_CHECK_ARG(h && codes && Wi && v && (D == 1 || pos_d), "rq_depth_input_fwd: null pointer argument");
   rq_depth_input_fwd_kernel<<<rq_grid(nseq * D, 8), 256, 0, stream>>>(h, codes, Wi, pos_d, v, nseq, D, C, Vi);
@@ -524,8 +537,9 @@ static int depth_common_bwd(const float* g, float* gh, float* gpos_d, long long 
   return 0;
 }
 
-int rq_depth_input_backward(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq, int D, int C,
-                            int Vi, cudaStream_t stream) {
+extern "C" int b200vq_rq_depth_input_bwd(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq,
+                                         int D, int C, int Vi, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = depth_shape_ok(nseq, D, C, Vi, "rq_depth_input_bwd")) return rc;
   B200_CHECK_ARG(codes && g && gh && gWi && (D == 1 || gpos_d), "rq_depth_input_bwd: null pointer argument");
   B200_CUDA_OK(cudaMemsetAsync(gWi, 0, (size_t)Vi * C * sizeof(float), stream));
@@ -538,18 +552,20 @@ int rq_depth_input_backward(const long long* codes, const float* g, float* gh, f
   return reverse_scan_rows(gWi, Vi, C, stream);
 }
 
-size_t rq_depth_input_bwd_deterministic_workspace_bytes(long long nseq, int D, int C, int Vi) {
+extern "C" size_t b200vq_rq_depth_input_bwd_deterministic_workspace_bytes(long long nseq, int D, int C, int Vi) {
   if (nseq <= 0 || D < 2 || C <= 0 || Vi <= 0) return 0;
   const long long N = nseq * (D - 1);
   return align256((size_t)N * sizeof(long long)) + scatter_det_workspace_bytes(N, Vi, C, kScatterRunToken);
 }
 
-int rq_depth_input_backward_deterministic(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d, long long nseq,
-                                          int D, int C, int Vi, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_rq_depth_input_bwd_deterministic(const long long* codes, const float* g, float* gh, float* gWi, float* gpos_d,
+                                                       long long nseq, int D, int C, int Vi, void* workspace, size_t ws_bytes,
+                                                       void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = depth_shape_ok(nseq, D, C, Vi, "rq_depth_input_bwd_deterministic")) return rc;
   B200_CHECK_ARG(codes && g && gh && gWi && (D == 1 || (gpos_d && workspace)), "rq_depth_input_bwd_deterministic: null pointer argument");
   B200_CHECK_ARG(nseq * D <= (1LL << 30), "rq_depth_input_bwd_deterministic: too many tokens");
-  B200_CHECK_ARG(ws_bytes >= rq_depth_input_bwd_deterministic_workspace_bytes(nseq, D, C, Vi),
+  B200_CHECK_ARG(ws_bytes >= b200vq_rq_depth_input_bwd_deterministic_workspace_bytes(nseq, D, C, Vi),
                  "rq_depth_input_bwd_deterministic: workspace too small");
   if (D > 1) {
     const long long N = nseq * (D - 1);
@@ -567,8 +583,9 @@ int rq_depth_input_backward_deterministic(const long long* codes, const float* g
   return reverse_scan_rows(gWi, Vi, C, stream);
 }
 
-int code_sum_embed(const long long* codes, long long ld, int n, const float* Wi, const float* pos, float* out, int B, int C, int Vi,
-                   cudaStream_t stream) {
+extern "C" int b200vq_code_sum_embed(const long long* codes, long long ld, int n, const float* Wi, const float* pos, float* out,
+                                     int B, int C, int Vi, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(codes && Wi && pos && out, "code_sum_embed: null pointer argument");
   B200_CHECK_ARG(B > 0 && C > 0 && C % 4 == 0 && Vi > 0 && n >= 1 && ld >= n, "code_sum_embed: bad shape (B=%d n=%d ld=%lld C=%d)", B, n,
                  ld, C);
@@ -576,5 +593,3 @@ int code_sum_embed(const long long* codes, long long ld, int n, const float* Wi,
   B200_LAUNCH_OK("code_sum_embed_kernel");
   return 0;
 }
-
-}  // namespace b200

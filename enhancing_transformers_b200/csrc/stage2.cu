@@ -9,6 +9,7 @@
 // All HBM-bound streams: float4 grid-stride loops, no shared-memory staging needed (every element is read once).
 // token_embed's backward scatters the table gradients with float atomics, or, on request, sums them in a fixed order
 // through scatter_det.cu (bit-reproducible).
+#include "../../include/b200vq.h"
 #include "common.cuh"
 #include "scatter_det.cuh"
 
@@ -236,8 +237,14 @@ decode_attention_kernel(const float* __restrict__ qkv, float* __restrict__ cache
   }
 }
 
+}  // namespace b200
+
 // ---------------------------------------------------------------------------------------------
-int time_mix_forward(const float* x, const float* w, float* y, long long M, int T, int C, int round_out, cudaStream_t stream) {
+using namespace b200;
+
+extern "C" int b200vq_time_mix_fwd(const float* x, const float* w, float* y, long long M, int T, int C, int round_out,
+                                   void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(M > 0 && T > 0 && C > 0 && C % 4 == 0 && M % T == 0, "time_mix: need C %% 4 == 0 and M %% T == 0 (M=%lld T=%d C=%d)", M, T, C);
   time_mix_fwd_kernel<<<s2_grid(M * (C / 4), 256), 256, 0, stream>>>(x, w, y, M, T, C / 4, round_out);
   B200_LAUNCH_OK("time_mix_fwd_kernel");
@@ -245,11 +252,14 @@ int time_mix_forward(const float* x, const float* w, float* y, long long M, int 
 }
 
 constexpr int kTimeMixRows = 64;
-size_t time_mix_bwd_workspace_bytes(long long M, int C) { return (size_t)((M + kTimeMixRows - 1) / kTimeMixRows) * C * sizeof(float); }
+extern "C" size_t b200vq_time_mix_bwd_workspace_bytes(long long M, int C) {
+  return (size_t)((M + kTimeMixRows - 1) / kTimeMixRows) * C * sizeof(float);
+}
 
 // gw_part [ceil(M/64), C]: summed over its rows (b200vq_colsum) it is the gradient of time_mix
-int time_mix_backward(const float* g, const float* x, const float* w, float* gx, float* gw_part, long long M, int T, int C,
-                      cudaStream_t stream) {
+extern "C" int b200vq_time_mix_bwd(const float* g, const float* x, const float* w, float* gx, float* gw_part, long long M, int T,
+                                   int C, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(M > 0 && T > 0 && C > 0 && C % 4 == 0 && M % T == 0, "time_mix: need C %% 4 == 0 and M %% T == 0 (M=%lld T=%d C=%d)", M, T, C);
   const long long chunks = (M + kTimeMixRows - 1) / kTimeMixRows;
   B200_CHECK_ARG(chunks <= 65535, "time_mix_backward: too many rows (%lld)", M);
@@ -259,7 +269,8 @@ int time_mix_backward(const float* g, const float* x, const float* w, float* gx,
   return 0;
 }
 
-int sqrelu(const float* x, const float* g, float* y, long long n, int grad, int round_out, cudaStream_t stream) {
+extern "C" int b200vq_sqrelu(const float* x, const float* g, float* y, long long n, int grad, int round_out, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(n > 0 && n % 4 == 0, "sqrelu: n %% 4");
   B200_CHECK_ARG(!grad || g, "sqrelu: the derivative form needs the incoming gradient");
   sqrelu_kernel<<<s2_grid(n / 4, 256), 256, 0, stream>>>(x, g, y, n / 4, grad, round_out);
@@ -267,8 +278,10 @@ int sqrelu(const float* x, const float* g, float* y, long long n, int grad, int 
   return 0;
 }
 
-int token_embed_forward(const long long* conds, const long long* codes, const float* Wc, const float* pos_c, const float* Wi,
-                        const float* pos_i, float* x, int B, int Tc, int Ti, int C, int Vc, int Vi, cudaStream_t stream) {
+extern "C" int b200vq_token_embed_fwd(const long long* conds, const long long* codes, const float* Wc, const float* pos_c,
+                                      const float* Wi, const float* pos_i, float* x, int B, int Tc, int Ti, int C, int Vc, int Vi,
+                                      void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && Tc >= 0 && Ti >= 0 && Tc + Ti > 0 && C > 0 && C % 4 == 0, "token_embed: bad shape B=%d Tc=%d Ti=%d C=%d", B, Tc, Ti, C);
   token_embed_fwd_kernel<<<s2_grid((long long)B * (Tc + Ti) * (C / 4), 256), 256, 0, stream>>>(conds, codes, Wc, pos_c, Wi, pos_i, x, B,
                                                                                               Tc, Ti, C / 4, Vc, Vi);
@@ -276,8 +289,9 @@ int token_embed_forward(const long long* conds, const long long* codes, const fl
   return 0;
 }
 
-int token_embed_backward(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c, float* gWi,
-                         float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, cudaStream_t stream) {
+extern "C" int b200vq_token_embed_bwd(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
+                                      float* gWi, float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && Tc >= 0 && Ti >= 0 && Tc + Ti > 0 && C > 0, "token_embed: bad shape B=%d Tc=%d Ti=%d C=%d", B, Tc, Ti, C);
   B200_CUDA_OK(cudaMemsetAsync(gWc, 0, (size_t)Vc * C * sizeof(float), stream));
   B200_CUDA_OK(cudaMemsetAsync(gWi, 0, (size_t)Vi * C * sizeof(float), stream));
@@ -288,22 +302,23 @@ int token_embed_backward(const long long* conds, const long long* codes, const f
 }
 
 // one scatter workspace, reused by the two tables in turn
-size_t token_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int Ti, int C, int Vc, int Vi) {
+extern "C" size_t b200vq_token_embed_bwd_deterministic_workspace_bytes(int B, int Tc, int Ti, int C, int Vc, int Vi) {
   if (B <= 0 || Tc < 0 || Ti < 0 || C <= 0) return 0;
   const size_t wc = Vc > 0 ? scatter_det_workspace_bytes((long long)B * Tc, Vc, C, kScatterRunToken) : 0;
   const size_t wi = Vi > 0 ? scatter_det_workspace_bytes((long long)B * Ti, Vi, C, kScatterRunToken) : 0;
   return wc > wi ? wc : wi;
 }
 
-int token_embed_backward_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc, float* gpos_c,
-                                       float* gWi, float* gpos_i, int B, int Tc, int Ti, int C, int Vc, int Vi, void* workspace,
-                                       size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_token_embed_bwd_deterministic(const long long* conds, const long long* codes, const float* g, float* gWc,
+                                                    float* gpos_c, float* gWi, float* gpos_i, int B, int Tc, int Ti, int C, int Vc,
+                                                    int Vi, void* workspace, size_t ws_bytes, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && Tc >= 0 && Ti >= 0 && Tc + Ti > 0 && C > 0, "token_embed: bad shape B=%d Tc=%d Ti=%d C=%d", B, Tc, Ti, C);
   B200_CHECK_ARG(Vc > 0 && Vi > 0, "token_embed: vocabulary sizes must be positive (Vc=%d Vi=%d)", Vc, Vi);
   B200_CHECK_ARG((long long)B * (Tc + Ti) <= (1LL << 30), "token_embed: too many tokens");
   B200_CHECK_ARG(g && gWc && gWi && (Tc == 0 || (conds && gpos_c)) && (Ti == 0 || (codes && gpos_i)) && workspace,
                  "token_embed_bwd_deterministic: null pointer argument");
-  B200_CHECK_ARG(ws_bytes >= token_embed_bwd_deterministic_workspace_bytes(B, Tc, Ti, C, Vc, Vi),
+  B200_CHECK_ARG(ws_bytes >= b200vq_token_embed_bwd_deterministic_workspace_bytes(B, Tc, Ti, C, Vc, Vi),
                  "token_embed_bwd_deterministic: workspace too small");
   const long long T = Tc + Ti;
   int rc = scatter_rows_det<kScatterRunToken>(conds, (long long)B * Tc, Vc, g, Tc, T, 0, C, gWc, workspace, ws_bytes, stream);
@@ -315,7 +330,9 @@ int token_embed_backward_deterministic(const long long* conds, const long long* 
   return 0;
 }
 
-int copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, int off_src, int off_dst, int n, int C, cudaStream_t stream) {
+extern "C" int b200vq_copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, int off_src, int off_dst, int n, int C,
+                                void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && T_src > 0 && T_dst > 0 && C > 0 && C % 4 == 0, "copy_rows: bad shape");
   B200_CHECK_ARG(n >= 0 && off_src >= 0 && off_dst >= 0 && off_src + n <= T_src && off_dst + n <= T_dst,
                  "copy_rows: window [%d, %d) / [%d, %d) outside the tensors", off_src, off_src + n, off_dst, off_dst + n);
@@ -324,8 +341,9 @@ int copy_rows(const float* src, float* dst, int B, int T_src, int T_dst, int off
   return 0;
 }
 
-int decode_attention(const float* qkv, float* cache_k, float* cache_v, float* out, int B, int heads, int hs, int Tmax, int pos,
-                     float scale, cudaStream_t stream) {
+extern "C" int b200vq_decode_attention(const float* qkv, float* cache_k, float* cache_v, float* out, int B, int heads, int hs,
+                                       int Tmax, int pos, float scale, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(B > 0 && heads > 0 && (hs == 32 || hs == 64), "decode_attention: head size must be 32 or 64 (got %d)", hs);
   B200_CHECK_ARG(pos >= 0 && pos < Tmax, "decode_attention: position %d outside the cache (%d rows)", pos, Tmax);
   B200_CHECK_ARG(B <= 65535, "decode_attention: batch too large");
@@ -337,5 +355,3 @@ int decode_attention(const float* qkv, float* cache_k, float* cache_v, float* ou
   B200_LAUNCH_OK("decode_attention_kernel");
   return 0;
 }
-
-}  // namespace b200

@@ -15,6 +15,7 @@
 //   vq_bwd  : closed-form gradients (see oracle/vitvq_oracle.py:vq_backward_np).  The codebook gradient is scattered with
 //             float atomics (vq_bwd_kernel) or, on request, stored per entry and summed in a fixed order
 //             (vq_bwd_contrib_kernel + scatter_det.cu): bit-reproducible.
+#include "../../include/b200vq.h"
 #include "common.cuh"
 #include "scatter_det.cuh"
 
@@ -523,17 +524,22 @@ constexpr size_t kVqSmemBytes =
     sizeof(float) * (kVqD * kVqTileM + 2 * kVqD * kVqTileN + 2 * kVqTileN + kVqTileM + kVqTileM + kVqThreads / 32) +
     sizeof(float4) * 8 * kVqThreads;
 
-size_t vq_workspace_bytes(int M, int K, int depth) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" size_t b200vq_vq_workspace_bytes(int M, int K, int depth) {
   const size_t nblk = (M + kVqTileM - 1) / kVqTileM;
   return ((size_t)kVqD * K + K + (size_t)depth * nblk) * sizeof(float);
 }
 
-int vq_forward(const float* z, const float* E, float* out, long long* idx, float* loss, int M, int K, int D, int depth,
-               float beta, int use_norm, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_vq_fwd(const float* z, const float* E, float* out, long long* idx, float* loss, int M, int K, int D, int depth,
+                             float beta, int use_norm, void* workspace, size_t ws_bytes, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
   B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d]", kVqMaxDepth);
-  B200_CHECK_ARG(ws_bytes >= vq_workspace_bytes(M, K, depth), "vq: workspace too small");
+  B200_CHECK_ARG(ws_bytes >= b200vq_vq_workspace_bytes(M, K, depth), "vq: workspace too small");
   float* EnT = static_cast<float*>(workspace);
   float* ee = EnT + (size_t)kVqD * K;
   float* part = ee + K;
@@ -549,8 +555,9 @@ int vq_forward(const float* z, const float* E, float* out, long long* idx, float
   return 0;
 }
 
-int vq_backward(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss, float* gz,
-                float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm, cudaStream_t stream) {
+extern "C" int b200vq_vq_bwd(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss, float* gz,
+                             float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
   B200_CHECK_ARG(M > 0 && M % 4 == 0, "vq: need M %% 4 == 0");
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: bad depth");
@@ -564,21 +571,22 @@ int vq_backward(const float* z, const float* E, const long long* idx, const floa
 }
 
 // contributions [M * depth, 32], then the scatter's own scratch
-size_t vq_bwd_deterministic_workspace_bytes(int M, int K, int D, int depth) {
+extern "C" size_t b200vq_vq_bwd_deterministic_workspace_bytes(int M, int K, int D, int depth) {
   if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || D != kVqD) return 0;
   const long long n = (long long)M * depth;
   const size_t contrib = ((size_t)n * kVqD * sizeof(float) + 255) & ~size_t(255);
   return contrib + scatter_det_workspace_bytes(n, K, kVqD, kScatterRunVq);
 }
 
-int vq_backward_deterministic(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss,
-                              float* gz, float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm,
-                              void* workspace, size_t ws_bytes, cudaStream_t stream) {
+extern "C" int b200vq_vq_bwd_deterministic(const float* z, const float* E, const long long* idx, const float* g_out,
+                                           const float* g_loss, float* gz, float* gE, int M, int K, int D, int depth, int residual,
+                                           float beta, int use_norm, void* workspace, size_t ws_bytes, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
   B200_CHECK_ARG(M > 0 && M % 4 == 0 && K > 0 && K % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
   B200_CHECK_ARG(z && E && idx && gz && gE && workspace, "vq_bwd_deterministic: null pointer argument");
-  B200_CHECK_ARG(ws_bytes >= vq_bwd_deterministic_workspace_bytes(M, K, D, depth), "vq_bwd_deterministic: workspace too small");
+  B200_CHECK_ARG(ws_bytes >= b200vq_vq_bwd_deterministic_workspace_bytes(M, K, D, depth), "vq_bwd_deterministic: workspace too small");
   const long long n = residual ? (long long)M * depth : M;   // entries: the plain quantiser reads idx[m]
   float* contrib = static_cast<float*>(workspace);
   const size_t contrib_bytes = ((size_t)M * depth * kVqD * sizeof(float) + 255) & ~size_t(255);
@@ -589,8 +597,9 @@ int vq_backward_deterministic(const float* z, const float* E, const long long* i
                                          ws_bytes - contrib_bytes, stream);
 }
 
-int vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
-             cudaStream_t stream) {
+extern "C" int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
+                               void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d", kVqD);
   B200_CHECK_ARG(M > 0 && M % 4 == 0 && depth >= 1, "vq_embed: bad sizes");
   vq_embed_kernel<<<(M * 8 + 255) / 256, 256, 0, stream>>>(E, codes, out, M, K, depth, use_norm);
@@ -600,6 +609,8 @@ int vq_embed(const float* E, const long long* codes, float* out, int M, int K, i
 
 // ---------------------------------------------------------------------------------------------
 // EMA codebook (van den Oord et al. 2017, appendix A.1, in the form of Taming Transformers' EMAVectorQuantizer)
+namespace b200 {
+
 __global__ void vq_counts_to_float_kernel(const int* __restrict__ icounts, float* __restrict__ counts, int K) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k < K) counts[k] = (float)icounts[k];    // exact: a count never exceeds M * depth < 2^24 (checked by the host)
@@ -641,12 +652,14 @@ vq_ema_weight_kernel(const float* __restrict__ cluster_size, const float* __rest
   }
 }
 
+}  // namespace b200
+
 static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 
-// [EnT | ee | loss parts] as vq_forward, [int counts K], deterministic: [contributions M*depth x 32 | scatter scratch]
-size_t vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int deterministic) {
+// [EnT | ee | loss parts] as b200vq_vq_fwd, [int counts K], deterministic: [contributions M*depth x 32 | scatter scratch]
+extern "C" size_t b200vq_vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int deterministic) {
   if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || D != kVqD) return 0;
-  size_t b = align256(vq_workspace_bytes(M, K, depth)) + align256((size_t)K * sizeof(int));
+  size_t b = align256(b200vq_vq_workspace_bytes(M, K, depth)) + align256((size_t)K * sizeof(int));
   if (deterministic) {
     const long long n = (long long)M * depth;
     b += align256((size_t)n * kVqD * sizeof(float)) + scatter_det_workspace_bytes(n, K, kVqD, kScatterRunVq);
@@ -654,21 +667,22 @@ size_t vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int determinis
   return b;
 }
 
-int vq_forward_ema(const float* z, const float* E, float* out, long long* idx, float* loss, float* counts, float* sums, int M, int K,
-                   int D, int depth, float beta, int use_norm, int deterministic, void* workspace, size_t ws_bytes,
-                   cudaStream_t stream) {
+extern "C" int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, long long* idx, float* loss, float* counts, float* sums,
+                                 int M, int K, int D, int depth, float beta, int use_norm, int deterministic, void* workspace,
+                                 size_t ws_bytes, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D == kVqD, "vq_fwd_ema: embed_dim must be %d (got %d)", kVqD, D);
   B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq_fwd_ema: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq_fwd_ema: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
   B200_CHECK_ARG(z && E && out && idx && loss && workspace, "vq_fwd_ema: null pointer argument");
   B200_CHECK_ARG((counts == nullptr) == (sums == nullptr), "vq_fwd_ema: counts and sums must both be given or both be NULL");
   B200_CHECK_ARG((long long)M * depth < (1ll << 24), "vq_fwd_ema: M * depth must be below 2^24 (fp32 counts stay exact)");
-  B200_CHECK_ARG(ws_bytes >= vq_fwd_ema_workspace_bytes(M, K, D, depth, deterministic), "vq_fwd_ema: workspace too small");
+  B200_CHECK_ARG(ws_bytes >= b200vq_vq_fwd_ema_workspace_bytes(M, K, D, depth, deterministic), "vq_fwd_ema: workspace too small");
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   float* EnT = reinterpret_cast<float*>(ws);
   float* ee = EnT + (size_t)kVqD * K;
   float* part = ee + K;
-  ws += align256(vq_workspace_bytes(M, K, depth));
+  ws += align256(b200vq_vq_workspace_bytes(M, K, depth));
   int* icounts = reinterpret_cast<int*>(ws);
   ws += align256((size_t)K * sizeof(int));
   float* contrib = reinterpret_cast<float*>(ws);
@@ -710,8 +724,9 @@ int vq_forward_ema(const float* z, const float* E, float* out, long long* idx, f
   return 0;
 }
 
-int vq_ema_update(const float* counts, const float* sums, float* cluster_size, float* embed_avg, float* weight, int K, int D,
-                  float decay, float eps, cudaStream_t stream) {
+extern "C" int b200vq_vq_ema_update(const float* counts, const float* sums, float* cluster_size, float* embed_avg, float* weight,
+                                    int K, int D, float decay, float eps, void* streamv) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   B200_CHECK_ARG(D == kVqD, "vq_ema_update: embed_dim must be %d (got %d)", kVqD, D);
   B200_CHECK_ARG(K > 0, "vq_ema_update: n_embed must be positive (got %d)", K);
   B200_CHECK_ARG(counts && sums && cluster_size && embed_avg && weight, "vq_ema_update: null pointer argument");
@@ -725,5 +740,3 @@ int vq_ema_update(const float* counts, const float* sums, float* cluster_size, f
   B200_LAUNCH_OK("vq_ema_weight_kernel");
   return 0;
 }
-
-}  // namespace b200
