@@ -36,6 +36,7 @@ _SIGNATURES = {
     "b200vq_attention_exact_fwd": (c_i, [c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_fl, c_f]),
     "b200vq_attention_exact_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_fl, c_f]),
     "b200vq_vq_workspace_bytes": (c_sz, [c_i, c_i, c_i]),
+    "b200vq_vq_fwd_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i]),
     "b200vq_vq_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_fl, c_i, c_f, c_sz, c_f]),
     "b200vq_vq_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_i, c_i, c_i, c_i, c_i, c_fl, c_i, c_f]),
     "b200vq_vq_bwd_deterministic_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i]),

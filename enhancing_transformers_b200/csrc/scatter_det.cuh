@@ -8,7 +8,7 @@
 
 namespace b200 {
 
-constexpr int kScatterRunVq = 128;      // 32-float codebook rows: up to M * depth entries, often on a few dozen ids
+constexpr int kScatterRunVq = 128;      // D-float codebook rows: up to M * depth entries, often on a few dozen ids
 constexpr int kScatterRunToken = 32;    // C-float embedding rows: B * T entries
 
 size_t scatter_det_workspace_bytes(long long N, int V, int C, int R);

@@ -21,7 +21,7 @@
 
 namespace b200 {
 
-constexpr int kVqD = 32;          // embed_dim of every shipped config (configs/*.yaml quantizer.embed_dim)
+constexpr int kVqD = 32;          // embed_dim of every shipped config (configs/*.yaml quantizer.embed_dim); wider: *_wide_kernel
 constexpr int kVqTileM = 128;     // tokens per CTA
 constexpr int kVqTileN = 128;     // codes per smem chunk
 constexpr int kVqThreads = 256;
@@ -524,6 +524,486 @@ constexpr size_t kVqSmemBytes =
     sizeof(float) * (kVqD * kVqTileM + 2 * kVqD * kVqTileN + 2 * kVqTileN + kVqTileM + kVqTileM + kVqThreads / 32) +
     sizeof(float4) * 8 * kVqThreads;
 
+// =============================================================================================
+// Wide codes: D = 32 * S for S in [2, 8] (D = 64 .. 256; RQ-VAE quantises 256-wide features).  The D = 32 kernels above
+// are not touched; the entry points pick these for D > 32.  Same arithmetic contract: distances fmaf(-2, dot, |z|^2 +
+// |e|^2) with dot summed by fmaf in ascending k, lowest index among equal distances, straight-through z + (acc - z),
+// normalisation by true division by max(|x|, 1e-12).
+//   - A row's squared norm is one thread's fmaf chain in column order (vq_row_sq): the lookup's phase A, its gather,
+//     vq_prep and vq_embed all normalise a row with the same bits, so vq_embed equals the lookup's accumulated code.
+//   - The lookup keeps the whole normalised tile zT [D][128] in shared memory and streams E^T through a two-stage ring
+//     in 32-row k-slices; the 8 x 8 accumulator tile stays in registers across a chunk's S slices, so every dot still
+//     sums k in order.  Phases A and C run one thread per token, so the transposed stores to zT are conflict-free.
+//   - The raw residual of the depth loop lives in a global workspace [M, D] (L2-resident at the shapes this serves) and
+//     the accumulated code in `out` itself, which the last depth overwrites with the straight-through value.
+//   - EMA statistics: the same 128-slot table keyed by code, filled one 32-column slice of the sums at a time.
+//   - Backward: one warp per token, lanes over columns; the per-token routine recomputes the depth recursion column by
+//     column in a few passes instead of holding depth x D values per lane, and is shared by the atomic and the
+//     deterministic kernel, so their gz agree bit for bit.
+constexpr int kVqSlice = 32;
+constexpr int kVqMaxD = 256;
+__host__ __device__ constexpr bool vq_width_ok(int D) { return D >= kVqSlice && D <= kVqMaxD && D % kVqSlice == 0; }
+
+__device__ __forceinline__ float vq_row_sq(const float* __restrict__ row, int D) {
+  float s = 0.f;
+  for (int c = 0; c < D; c += 4) {
+    const float4 v = *reinterpret_cast<const float4*>(row + c);
+    s = fmaf(v.x, v.x, s); s = fmaf(v.y, v.y, s); s = fmaf(v.z, v.z, s); s = fmaf(v.w, v.w, s);
+  }
+  return s;
+}
+__device__ __forceinline__ float vq_row_norm(const float* __restrict__ row, int D, int use_norm) {
+  return use_norm ? fmaxf(sqrtf(vq_row_sq(row, D)), kNormEps) : 1.f;   // x / 1 == x: use_norm == 0 divides by 1
+}
+__device__ __forceinline__ float4 div4(const float4& v, float n) { return make_float4(v.x / n, v.y / n, v.z / n, v.w / n); }
+
+// one thread per code: EnT [D][K] (coalesced across the warp's codes), ee [K]
+__global__ void vq_prep_wide_kernel(const float* __restrict__ E, float* __restrict__ EnT, float* __restrict__ ee, int K, int D,
+                                    int use_norm) {
+  const int code = blockIdx.x * blockDim.x + threadIdx.x;
+  if (code >= K) return;
+  const float* row = E + (size_t)code * D;
+  const float nrm = vq_row_norm(row, D, use_norm);
+  float s2 = 0.f;
+  for (int c = 0; c < D; c += 4) {
+    const float4 v = div4(*reinterpret_cast<const float4*>(row + c), nrm);
+    EnT[(size_t)(c + 0) * K + code] = v.x;
+    EnT[(size_t)(c + 1) * K + code] = v.y;
+    EnT[(size_t)(c + 2) * K + code] = v.z;
+    EnT[(size_t)(c + 3) * K + code] = v.w;
+    s2 = fmaf(v.x, v.x, s2); s2 = fmaf(v.y, v.y, s2); s2 = fmaf(v.z, v.z, s2); s2 = fmaf(v.w, v.w, s2);
+  }
+  ee[code] = s2;
+}
+
+struct VqWideStatTable {
+  int keys[kVqStatSlots];
+  int cnt[kVqStatSlots];
+  int slot[kVqTileM];                    // the slot of each of the CTA's tokens (-1: dead token)
+  float acc[kVqStatSlots][kVqSlice];     // one 32-column slice of the sums
+};
+
+__host__ __device__ constexpr size_t vq_wide_smem_bytes(int D, bool stats) {
+  return sizeof(float) * ((size_t)D * kVqTileM + 2 * kVqSlice * kVqTileN + 2 * kVqTileN + kVqTileM + kVqTileM + kVqThreads / 32) +
+         sizeof(int) * 8 * kVqThreads + (stats ? sizeof(VqWideStatTable) : 0);
+}
+
+// z [M,D]; EnT [D][K]; ee [K]; E [K,D]; out [M,D] (holds the accumulated code between depths); rws [M,D] raw residual
+// (depth > 1 only); idx [M,depth]; loss_part [depth][gridDim.x]; statistics as vq_fwd_kernel with D-wide rows
+template <int kStats>
+__global__ void __launch_bounds__(kVqThreads, 2)
+vq_fwd_wide_kernel(const float* __restrict__ z, const float* __restrict__ EnT, const float* __restrict__ ee,
+                   const float* __restrict__ E, float* __restrict__ out, float* __restrict__ rws, long long* __restrict__ idx_out,
+                   float* __restrict__ loss_part, int M, int K, int D, int depth, int use_norm, int* __restrict__ counts,
+                   float* __restrict__ sums, float* __restrict__ contrib) {
+  extern __shared__ __align__(16) uint8_t vq_smem[];
+  float (*zT)[kVqTileM] = reinterpret_cast<float (*)[kVqTileM]>(vq_smem);
+  float (*eT)[kVqSlice][kVqTileN] = reinterpret_cast<float (*)[kVqSlice][kVqTileN]>(vq_smem + sizeof(float) * D * kVqTileM);
+  float (*ee_s)[kVqTileN] = reinterpret_cast<float (*)[kVqTileN]>(eT + 2);
+  float* zz_s = reinterpret_cast<float*>(ee_s + 2);
+  int* best_s = reinterpret_cast<int*>(zz_s + kVqTileM);
+  float* red_s = reinterpret_cast<float*>(best_s + kVqTileM);
+  // each thread's 8 running argmin indices, [i][tid]: only stored when a distance improves and read once per depth, so
+  // the 8 registers they would take stay with the accumulator tile (128 per thread for two CTAs per SM, no spills)
+  int (*besti)[kVqThreads] = reinterpret_cast<int (*)[kVqThreads]>(red_s + kVqThreads / 32);
+  VqWideStatTable* st = reinterpret_cast<VqWideStatTable*>(besti + 8);   // kStats != 0 only
+
+  const int tid = threadIdx.x;
+  const int m0 = blockIdx.x * kVqTileM;
+  const int lt = tid, tok = m0 + tid;                 // phases A and C: one thread per token (threads < 128)
+  const bool row_thread = tid < kVqTileM, live = row_thread && tok < M;
+  const int tx = tid & 15, ty = tid >> 4;             // phase B: 16 x 16 threads, 8 tokens x 8 codes each
+  const int S = D / kVqSlice;
+  const int nchunks = (K + kVqTileN - 1) / kVqTileN;
+  const int nsteps = nchunks * S;
+  if constexpr (kStats != kVqStatsOff) {
+    for (int i = tid; i < kVqStatSlots; i += kVqThreads) { st->keys[i] = -1; st->cnt[i] = 0; }
+#pragma unroll 1
+    for (int i = tid; i < kVqStatSlots * kVqSlice; i += kVqThreads) (&st->acc[0][0])[i] = 0.f;
+  }
+
+  for (int t = 0; t < depth; ++t) {
+    const float* src = (t == 0 ? z : rws) + (size_t)tok * D;    // the raw residual entering depth t
+    // ---- phase A: normalise the residual, stage it transposed -------------------------------
+    if (row_thread) {
+      float s2 = 0.f;
+      if (live) {
+        const float nrm = vq_row_norm(src, D, use_norm);
+        for (int c = 0; c < D; c += 4) {
+          const float4 v = div4(*reinterpret_cast<const float4*>(src + c), nrm);
+          zT[c + 0][lt] = v.x; zT[c + 1][lt] = v.y; zT[c + 2][lt] = v.z; zT[c + 3][lt] = v.w;
+          s2 = fmaf(v.x, v.x, s2); s2 = fmaf(v.y, v.y, s2); s2 = fmaf(v.z, v.z, s2); s2 = fmaf(v.w, v.w, s2);
+        }
+      } else {
+        for (int c = 0; c < D; ++c) zT[c][lt] = 0.f;
+      }
+      zz_s[lt] = s2;
+    }
+    // ---- phase B: distances + running argmin, E^T streamed in 32-row k-slices -----------------
+    auto load_slice = [&](int step, int buf) {
+      const int c = step / S, s = step - c * S;
+      const int c0 = c * kVqTileN;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int f = tid + i * kVqThreads;
+        const int row = f >> 5, col4 = (f & 31) * 4;
+        const bool ok = c0 + col4 < K;   // K % 4 == 0 enforced by the host
+        cp_async16(&eT[buf][row][col4], EnT + (size_t)(s * kVqSlice + row) * K + (ok ? c0 + col4 : 0), ok);
+      }
+      if (s == 0 && tid < kVqTileN / 4) {
+        const bool ok = c0 + tid * 4 < K;
+        cp_async16(&ee_s[c & 1][tid * 4], ee + (ok ? c0 + tid * 4 : 0), ok);
+      }
+      cp_async_commit();
+    };
+    float bestd[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { bestd[i] = INFINITY; besti[i][tid] = 0x7fffffff; }
+    float2 dacc[8][4];     // 8 tokens x 8 codes, kept across the chunk's slices
+    load_slice(0, 0);
+    for (int step = 0; step < nsteps; ++step) {
+      const int buf = step & 1;
+      const int c = step / S, s = step - c * S;
+      if (step + 1 < nsteps) { load_slice(step + 1, buf ^ 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
+      __syncthreads();   // slice `step` (and, for step 0, zT / zz_s) visible
+      if (s == 0) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) dacc[i][j] = make_float2(0.f, 0.f);
+      }
+      const float (*zs)[kVqTileM] = zT + s * kVqSlice;
+#pragma unroll 8
+      for (int k = 0; k < kVqSlice; ++k) {
+        const float4 za = *reinterpret_cast<const float4*>(&zs[k][ty * 4]);
+        const float4 zb = *reinterpret_cast<const float4*>(&zs[k][64 + ty * 4]);
+        const float4 ea = *reinterpret_cast<const float4*>(&eT[buf][k][tx * 4]);
+        const float4 eb = *reinterpret_cast<const float4*>(&eT[buf][k][64 + tx * 4]);
+        const float zv[8] = {za.x, za.y, za.z, za.w, zb.x, zb.y, zb.z, zb.w};
+        const float2 ev[4] = {make_float2(ea.x, ea.y), make_float2(ea.z, ea.w), make_float2(eb.x, eb.y), make_float2(eb.z, eb.w)};
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) ffma2(dacc[i][j], zv[i], ev[j]);
+      }
+      if (s == S - 1) {
+        const int c0 = c * kVqTileN;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float zz = zz_s[(i < 4 ? 0 : 64) + ty * 4 + (i & 3)];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int lc = (j < 4 ? 0 : 64) + tx * 4 + (j & 3);
+            const int code = c0 + lc;
+            const float dot = (j & 1) ? dacc[i][j >> 1].y : dacc[i][j >> 1].x;
+            const float d = fmaf(-2.f, dot, zz + ee_s[c & 1][lc]);
+            if (code < K && d < bestd[i]) { bestd[i] = d; besti[i][tid] = code; }
+          }
+        }
+      }
+      __syncthreads();   // everyone done with buf before it is refilled
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      int bi = besti[i][tid];
+#pragma unroll
+      for (int o = 1; o < 16; o <<= 1) {
+        const float od = __shfl_xor_sync(0xffffffffu, bestd[i], o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (od < bestd[i] || (od == bestd[i] && oi < bi)) { bestd[i] = od; bi = oi; }
+      }
+      if (tx == 0) best_s[(i < 4 ? 0 : 64) + ty * 4 + (i & 3)] = bi;
+    }
+    __syncthreads();
+    // ---- phase C: gather, normalise, loss, residual and accumulated code ------------------------
+    float lsum = 0.f;
+    if (live) {
+      int code = best_s[lt];
+      if (code >= K) code = 0;   // only for rows of NaNs: torch.argmin would also return some index
+      const float* er = E + (size_t)code * D;
+      const float ne = vq_row_norm(er, D, use_norm);
+      float* orow = out + (size_t)tok * D;
+      const float* zrow = z + (size_t)tok * D;
+      float* rrow = rws + (size_t)tok * D;
+      for (int c = 0; c < D; c += 4) {
+        const float4 q = div4(*reinterpret_cast<const float4*>(er + c), ne);
+        const float dx = q.x - zT[c + 0][lt], dy = q.y - zT[c + 1][lt], dz = q.z - zT[c + 2][lt], dw = q.w - zT[c + 3][lt];
+        lsum = fmaf(dx, dx, lsum); lsum = fmaf(dy, dy, lsum); lsum = fmaf(dz, dz, lsum); lsum = fmaf(dw, dw, lsum);
+        if (t + 1 < depth) {
+          float4 r = *reinterpret_cast<const float4*>(src + c);
+          r.x -= q.x; r.y -= q.y; r.z -= q.z; r.w -= q.w;
+          *reinterpret_cast<float4*>(rrow + c) = r;
+        }
+        float4 a = t == 0 ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(orow + c);
+        a.x += q.x; a.y += q.y; a.z += q.z; a.w += q.w;
+        if (t + 1 == depth) {
+          const float4 zr = *reinterpret_cast<const float4*>(zrow + c);
+          a = make_float4(zr.x + (a.x - zr.x), zr.y + (a.y - zr.y), zr.z + (a.z - zr.z), zr.w + (a.w - zr.w));
+        }
+        *reinterpret_cast<float4*>(orow + c) = a;
+      }
+      idx_out[(size_t)tok * depth + t] = code;
+    }
+    lsum = warp_sum(lsum);
+    if ((tid & 31) == 0) red_s[tid >> 5] = lsum;
+    __syncthreads();
+    if constexpr (kStats != kVqStatsOff) {
+      // zT still holds the vectors the lookup compared, best_s the codes
+      if (row_thread) {
+        int slot = -1;
+        if (live) {
+          int code = best_s[lt];
+          if (code >= K) code = 0;   // as phase C
+          unsigned h = ((unsigned)code * 2654435761u) >> 25;
+#pragma unroll 1
+          for (int probe = 0; probe < kVqStatSlots; ++probe) {
+            const int old = atomicCAS(&st->keys[h], -1, code);
+            if (old == -1 || old == code) { slot = (int)h; break; }
+            h = (h + 1) & (kVqStatSlots - 1);
+          }
+          atomicAdd(&st->cnt[slot], 1);
+          if (kStats == kVqStatsDeterministic) {
+            float* crow = contrib + ((size_t)tok * depth + t) * D;
+            for (int c = 0; c < D; c += 4)
+              *reinterpret_cast<float4*>(crow + c) = make_float4(zT[c][lt], zT[c + 1][lt], zT[c + 2][lt], zT[c + 3][lt]);
+          }
+        }
+        st->slot[lt] = slot;
+      }
+      __syncthreads();
+      if constexpr (kStats == kVqStatsAtomic) {
+#pragma unroll 1
+        for (int s = 0; s < S; ++s) {
+          if (row_thread && st->slot[lt] >= 0) {
+            float* acc = st->acc[st->slot[lt]];
+#pragma unroll 4
+            for (int j = 0; j < kVqSlice; ++j) {
+              const int col = (j + tid) & (kVqSlice - 1);    // lanes start on different banks
+              atomicAdd(acc + col, zT[s * kVqSlice + col][lt]);
+            }
+          }
+          __syncthreads();
+#pragma unroll 1
+          for (int i = tid; i < kVqStatSlots * kVqSlice; i += kVqThreads) {
+            const int slot = i / kVqSlice, col = i % kVqSlice;
+            const int key = st->keys[slot];
+            if (key >= 0) {
+              atomicAdd(sums + (size_t)key * D + s * kVqSlice + col, st->acc[slot][col]);
+              st->acc[slot][col] = 0.f;
+            }
+          }
+          __syncthreads();
+        }
+      }
+      // counts, then an empty table for the next depth (whose statistics follow phase B's barriers)
+      for (int i = tid; i < kVqStatSlots; i += kVqThreads) {
+        const int key = st->keys[i];
+        if (key >= 0) atomicAdd(counts + key, st->cnt[i]);
+        st->keys[i] = -1;
+        st->cnt[i] = 0;
+      }
+    }
+    if (tid == 0) {
+      float s = 0.f;
+      for (int w = 0; w < kVqThreads / 32; ++w) s += red_s[w];
+      loss_part[(size_t)t * gridDim.x + blockIdx.x] = s;
+    }
+  }
+}
+
+// Per-token closed-form gradients at width D, one warp per token (lane l owns columns l, l + 32, ...): writes gz's row
+// and hands every codebook contribution to claim(t, code) -> handle (once per depth step, warp-uniform) and
+// emit(handle, code, column, value).  The residual recursion r_{t+1} = r_t - q_t is recomputed column by column in each
+// pass (norms, then J^T dot products), so a lane holds O(depth) scalars instead of depth x D floats.
+template <class Claim, class Emit>
+__device__ __forceinline__ void vq_bwd_token_wide(const float* __restrict__ z, const float* __restrict__ E,
+                                                  const long long* __restrict__ idx, const float* __restrict__ g_out,
+                                                  float* __restrict__ gz, float g_loss, int tk, int lane, int M, int D,
+                                                  int depth, int residual, float beta, int use_norm, Claim&& claim, Emit&& emit) {
+  const float cc = 2.f / ((float)M * (float)D);
+  const float* zr = z + (size_t)tk * D;
+  auto nrm_of = [&](float s) { return use_norm ? fmaxf(sqrtf(warp_sum(s)), kNormEps) : 1.f; };
+  for (int c = lane; c < D; c += 32) gz[(size_t)tk * D + c] = g_out ? g_out[(size_t)tk * D + c] : 0.f;
+  if (!residual) {
+    const long long code = idx[tk];
+    const float* er = E + (size_t)code * D;
+    float sz = 0.f, se = 0.f;
+    for (int c = lane; c < D; c += 32) { sz = fmaf(zr[c], zr[c], sz); se = fmaf(er[c], er[c], se); }
+    const float nz = nrm_of(sz), ne = nrm_of(se);
+    float pz = 0.f, pe = 0.f;
+    for (int c = lane; c < D; c += 32) {
+      const float zn = zr[c] / nz, qn = er[c] / ne, d = zn - qn;
+      pz = fmaf(zn, d, pz);
+      pe = fmaf(qn, -d, pe);
+    }
+    pz = warp_sum(pz);
+    pe = warp_sum(pe);
+    const float sz_ = g_loss * beta * cc, se_ = g_loss * cc;
+    const int h = claim(0, code);
+    for (int c = lane; c < D; c += 32) {
+      const float zn = zr[c] / nz, qn = er[c] / ne, d = zn - qn;
+      const float jz = use_norm ? fmaf(-zn, pz, d) / nz : d;
+      const float je = use_norm ? fmaf(-qn, pe, -d) / ne : -d;
+      gz[(size_t)tk * D + c] = fmaf(sz_, jz, gz[(size_t)tk * D + c]);
+      emit(h, code, c, se_ * je);
+    }
+    return;
+  }
+  const float gl = g_loss / (float)depth;
+  const float s1 = gl * cc, s2 = gl * beta * cc;
+  int cd[kVqMaxDepth];                     // codes index K < 2^31 rows: an int, and E + cd * D recomputed, keep registers free
+  float ne[kVqMaxDepth], nr[kVqMaxDepth], pr[kVqMaxDepth], pq[kVqMaxDepth];
+  auto er = [&](int t, int c) { return E[(size_t)cd[t] * D + c]; };
+#pragma unroll
+  for (int t = 0; t < kVqMaxDepth; ++t) {
+    cd[t] = t < depth ? (int)idx[(size_t)tk * depth + t] : 0;
+    float se = 0.f;
+    if (t < depth)
+      for (int c = lane; c < D; c += 32) se = fmaf(er(t, c), er(t, c), se);
+    ne[t] = t < depth ? nrm_of(se) : 1.f;
+    pr[t] = 0.f; pq[t] = 0.f;
+  }
+  // |r_t|
+  {
+    float sr[kVqMaxDepth];
+#pragma unroll
+    for (int t = 0; t < kVqMaxDepth; ++t) sr[t] = 0.f;
+    for (int c = lane; c < D; c += 32) {
+      float r = zr[c];
+#pragma unroll
+      for (int t = 0; t < kVqMaxDepth; ++t)
+        if (t < depth) { sr[t] = fmaf(r, r, sr[t]); r -= er(t, c) / ne[t]; }
+    }
+#pragma unroll
+    for (int t = 0; t < kVqMaxDepth; ++t) nr[t] = t < depth ? nrm_of(sr[t]) : 1.f;
+  }
+  // rn_t . (rn_t - qn_t)
+  for (int c = lane; c < D; c += 32) {
+    float r = zr[c];
+#pragma unroll
+    for (int t = 0; t < kVqMaxDepth; ++t)
+      if (t < depth) {
+        const float rn = r / nr[t], qn = er(t, c) / ne[t];
+        pr[t] = fmaf(rn, rn - qn, pr[t]);
+        r -= qn;
+      }
+  }
+#pragma unroll
+  for (int t = 0; t < kVqMaxDepth; ++t) pr[t] = warp_sum(pr[t]);
+  // column c of tot_s = gq_s - sum_{t > s} gr_t for every depth s, handed to f(s, qn_s, tot_s)
+  auto column = [&](int c, auto&& f) {
+    float qn[kVqMaxDepth], gq[kVqMaxDepth], gr[kVqMaxDepth];
+    float r = zr[c];
+#pragma unroll
+    for (int t = 0; t < kVqMaxDepth; ++t)
+      if (t < depth) {
+        const float rn = r / nr[t];
+        qn[t] = er(t, c) / ne[t];
+        gq[t] = s1 * (qn[t] - rn);
+        const float d = rn - qn[t];
+        gr[t] = s2 * (use_norm ? fmaf(-rn, pr[t], d) / nr[t] : d);
+        r -= qn[t];
+      }
+    float suffix = 0.f;
+#pragma unroll
+    for (int s = kVqMaxDepth - 1; s >= 0; --s)
+      if (s < depth) {
+        f(s, qn[s], gq[s] - suffix);
+        suffix += gr[s];
+      }
+  };
+  for (int c = lane; c < D; c += 32) column(c, [&](int s, float qn, float tot) { pq[s] = fmaf(qn, tot, pq[s]); });
+  int h[kVqMaxDepth];
+#pragma unroll
+  for (int t = 0; t < kVqMaxDepth; ++t) {
+    pq[t] = warp_sum(pq[t]);
+    h[t] = t < depth ? claim(t, cd[t]) : -1;
+  }
+  for (int c = lane; c < D; c += 32)
+    column(c, [&](int s, float qn, float tot) { emit(h[s], cd[s], c, use_norm ? fmaf(-qn, pq[s], tot) / ne[s] : tot); });
+}
+
+// The atomic backward's table: slots x D floats (64 KB whatever D) keyed by code, probed by lane 0 of a token's warp.
+__host__ __device__ constexpr int vq_wide_bwd_slots(int D) { return 16384 / D; }
+__host__ __device__ constexpr size_t vq_wide_bwd_smem_bytes(int D) {
+  return (size_t)vq_wide_bwd_slots(D) * (sizeof(int) + sizeof(float) * D);
+}
+constexpr size_t kVqWideBwdSmemMax = vq_wide_bwd_smem_bytes(2 * kVqSlice);   // the narrowest wide code has the most keys
+
+// gz [M,D] (written), gE [K,D] (atomically accumulated; caller zero-fills)
+__global__ void __launch_bounds__(kVqBwdThreads)
+vq_bwd_wide_kernel(const float* __restrict__ z, const float* __restrict__ E, const long long* __restrict__ idx,
+                   const float* __restrict__ g_out, const float* __restrict__ g_loss_ptr, float* __restrict__ gz,
+                   float* __restrict__ gE, int M, int D, int depth, int residual, float beta, int use_norm) {
+  extern __shared__ __align__(16) uint8_t vq_smem[];
+  const int slots = vq_wide_bwd_slots(D);
+  float* acc = reinterpret_cast<float*>(vq_smem);
+  int* keys = reinterpret_cast<int*>(acc + (size_t)slots * D);
+  for (int i = threadIdx.x; i < slots; i += kVqBwdThreads) keys[i] = -1;
+  for (int i = threadIdx.x; i < slots * D; i += kVqBwdThreads) acc[i] = 0.f;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float g_loss = g_loss_ptr ? *g_loss_ptr : 0.f;
+  auto claim = [&](int, long long code) {
+    int slot = -1;
+    if (lane == 0) {
+      unsigned hh = (((unsigned)code * 2654435761u) >> 16) % (unsigned)slots;
+#pragma unroll 1
+      for (int probe = 0; probe < 8; ++probe) {
+        const int old = atomicCAS(&keys[hh], -1, (int)code);
+        if (old == -1 || old == (int)code) { slot = (int)hh; break; }
+        hh = hh + 1 == (unsigned)slots ? 0 : hh + 1;
+      }
+    }
+    return __shfl_sync(0xffffffffu, slot, 0);
+  };
+  auto emit = [&](int slot, long long code, int c, float v) {
+    atomicAdd(slot >= 0 ? &acc[(size_t)slot * D + c] : gE + (size_t)code * D + c, v);
+  };
+  for (int tk = blockIdx.x * (kVqBwdThreads / 32) + warp; tk < M; tk += gridDim.x * (kVqBwdThreads / 32))
+    vq_bwd_token_wide(z, E, idx, g_out, gz, g_loss, tk, lane, M, D, depth, residual, beta, use_norm, claim, emit);
+  __syncthreads();
+  for (int i = threadIdx.x; i < slots * D; i += kVqBwdThreads) {
+    const int key = keys[i / D];
+    if (key >= 0 && acc[i] != 0.f) atomicAdd(gE + (size_t)key * D + i % D, acc[i]);
+  }
+}
+
+// deterministic backward, first half: entry m * depth + t (m for the plain quantiser) stores its row in contrib [entries, D]
+__global__ void __launch_bounds__(kVqBwdThreads)
+vq_bwd_contrib_wide_kernel(const float* __restrict__ z, const float* __restrict__ E, const long long* __restrict__ idx,
+                           const float* __restrict__ g_out, const float* __restrict__ g_loss_ptr, float* __restrict__ gz,
+                           float* __restrict__ contrib, int M, int D, int depth, int residual, float beta, int use_norm) {
+  const int lane = threadIdx.x & 31;
+  const int tk = blockIdx.x * (kVqBwdThreads / 32) + (threadIdx.x >> 5);
+  if (tk >= M) return;    // whole warp
+  const float g_loss = g_loss_ptr ? *g_loss_ptr : 0.f;
+  vq_bwd_token_wide(z, E, idx, g_out, gz, g_loss, tk, lane, M, D, depth, residual, beta, use_norm,
+                    [&](int t, long long) { return residual ? tk * depth + t : tk; },
+                    [&](int entry, long long, int c, float v) { contrib[(size_t)entry * D + c] = v; });
+}
+
+// decode_codes at width D, one thread per token: the lookup's normalisation and accumulation order, so the result is
+// bit-identical to the accumulated code of vq_fwd_wide_kernel
+__global__ void vq_embed_wide_kernel(const float* __restrict__ E, const long long* __restrict__ codes, float* __restrict__ out, int M,
+                                     int K, int D, int depth, int use_norm) {
+  const int tok = blockIdx.x * blockDim.x + threadIdx.x;
+  if (tok >= M) return;
+  float* orow = out + (size_t)tok * D;
+  for (int t = 0; t < depth; ++t) {
+    long long code = codes[(size_t)tok * depth + t];
+    if (code < 0 || code >= K) code = 0;
+    const float* er = E + (size_t)code * D;
+    const float ne = vq_row_norm(er, D, use_norm);
+    for (int c = 0; c < D; c += 4) {
+      const float4 q = div4(*reinterpret_cast<const float4*>(er + c), ne);
+      float4 a = t == 0 ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(orow + c);
+      a.x += q.x; a.y += q.y; a.z += q.z; a.w += q.w;
+      *reinterpret_cast<float4*>(orow + c) = a;
+    }
+  }
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -533,24 +1013,72 @@ extern "C" size_t b200vq_vq_workspace_bytes(int M, int K, int depth) {
   return ((size_t)kVqD * K + K + (size_t)depth * nblk) * sizeof(float);
 }
 
+static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+
+extern "C" size_t b200vq_vq_fwd_workspace_bytes(int M, int K, int D, int depth) {
+  if (!vq_width_ok(D)) return 0;
+  if (D == kVqD) return b200vq_vq_workspace_bytes(M, K, depth);
+  // [EnT D x K | ee K | loss parts depth x blocks], then the raw residual [M, D] of the depth loop
+  const size_t nblk = (M + kVqTileM - 1) / kVqTileM;
+  const size_t base = ((size_t)D * K + K + (size_t)depth * nblk) * sizeof(float);
+  return depth > 1 ? align256(base) + (size_t)M * D * sizeof(float) : base;
+}
+
+// vq_prep + the lookup at D > 32 into the b200vq_vq_fwd_workspace_bytes layout; part receives the loss partial sums
+static int vq_lookup_wide(const float* z, const float* E, float* out, long long* idx, int M, int K, int D, int depth, int use_norm,
+                          int stats, int* icounts, float* sums, float* contrib, void* workspace, float** part, cudaStream_t stream) {
+  float* EnT = static_cast<float*>(workspace);
+  float* ee = EnT + (size_t)D * K;
+  *part = ee + K;
+  const int nblk = (M + kVqTileM - 1) / kVqTileM;
+  float* rws = depth > 1 ? reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) +
+                                                     align256(((size_t)D * K + K + (size_t)depth * nblk) * sizeof(float)))
+                         : nullptr;
+  vq_prep_wide_kernel<<<(K + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, D, use_norm);
+  B200_LAUNCH_OK("vq_prep_wide_kernel");
+  const size_t smem = vq_wide_smem_bytes(D, stats != kVqStatsOff);
+  if (stats == kVqStatsOff) {
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kVqStatsOff>, vq_wide_smem_bytes(kVqMaxD, false));
+    vq_fwd_wide_kernel<kVqStatsOff><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth,
+                                                                        use_norm, nullptr, nullptr, nullptr);
+  } else if (stats == kVqStatsAtomic) {
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kVqStatsAtomic>, vq_wide_smem_bytes(kVqMaxD, true));
+    vq_fwd_wide_kernel<kVqStatsAtomic><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth,
+                                                                           use_norm, icounts, sums, nullptr);
+  } else {
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kVqStatsDeterministic>, vq_wide_smem_bytes(kVqMaxD, true));
+    vq_fwd_wide_kernel<kVqStatsDeterministic><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, rws, idx, *part, M, K, D,
+                                                                                  depth, use_norm, icounts, nullptr, contrib);
+  }
+  B200_LAUNCH_OK("vq_fwd_wide_kernel");
+  return 0;
+}
+
 extern "C" int b200vq_vq_fwd(const float* z, const float* E, float* out, long long* idx, float* loss, int M, int K, int D, int depth,
                              float beta, int use_norm, void* workspace, size_t ws_bytes, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
   B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d]", kVqMaxDepth);
-  B200_CHECK_ARG(ws_bytes >= b200vq_vq_workspace_bytes(M, K, depth), "vq: workspace too small");
-  float* EnT = static_cast<float*>(workspace);
-  float* ee = EnT + (size_t)kVqD * K;
-  float* part = ee + K;
+  B200_CHECK_ARG(ws_bytes >= b200vq_vq_fwd_workspace_bytes(M, K, D, depth), "vq: workspace too small");
   const int nblk = (M + kVqTileM - 1) / kVqTileM;
-  vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
-  B200_LAUNCH_OK("vq_prep_kernel");
-  B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsOff>, kVqSmemBytes);
-  vq_fwd_kernel<kVqStatsOff><<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
-                                                                         nullptr, nullptr, nullptr);
-  B200_LAUNCH_OK("vq_fwd_kernel");
-  vq_loss_kernel<false><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)kVqD), beta, loss);
+  float* part;
+  if (D == kVqD) {
+    float* EnT = static_cast<float*>(workspace);
+    float* ee = EnT + (size_t)kVqD * K;
+    part = ee + K;
+    vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
+    B200_LAUNCH_OK("vq_prep_kernel");
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsOff>, kVqSmemBytes);
+    vq_fwd_kernel<kVqStatsOff><<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
+                                                                           nullptr, nullptr, nullptr);
+    B200_LAUNCH_OK("vq_fwd_kernel");
+  } else {
+    const int rc = vq_lookup_wide(z, E, out, idx, M, K, D, depth, use_norm, kVqStatsOff, nullptr, nullptr, nullptr, workspace, &part,
+                                  stream);
+    if (rc != 0) return rc;
+  }
+  vq_loss_kernel<false><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)D), beta, loss);
   B200_LAUNCH_OK("vq_loss_kernel");
   return 0;
 }
@@ -558,52 +1086,72 @@ extern "C" int b200vq_vq_fwd(const float* z, const float* E, float* out, long lo
 extern "C" int b200vq_vq_bwd(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss, float* gz,
                              float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
   B200_CHECK_ARG(M > 0 && M % 4 == 0, "vq: need M %% 4 == 0");
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: bad depth");
-  B200_CUDA_OK(cudaMemsetAsync(gE, 0, (size_t)K * kVqD * sizeof(float), stream));
-  int blocks = (M + 31) / 32;
+  B200_CUDA_OK(cudaMemsetAsync(gE, 0, (size_t)K * D * sizeof(float), stream));
   const int cap = num_sms() * 2;          // few, long-lived CTAs: each aggregates ~M / cap tokens in its table
+  if (D == kVqD) {
+    int blocks = (M + 31) / 32;
+    if (blocks > cap) blocks = cap;
+    vq_bwd_kernel<<<blocks, kVqBwdThreads, 0, stream>>>(z, E, idx, g_out, g_loss, gz, gE, M, K, depth, residual, beta, use_norm);
+    B200_LAUNCH_OK("vq_bwd_kernel");
+    return 0;
+  }
+  int blocks = (M + kVqBwdThreads / 32 - 1) / (kVqBwdThreads / 32);
   if (blocks > cap) blocks = cap;
-  vq_bwd_kernel<<<blocks, kVqBwdThreads, 0, stream>>>(z, E, idx, g_out, g_loss, gz, gE, M, K, depth, residual, beta, use_norm);
-  B200_LAUNCH_OK("vq_bwd_kernel");
+  B200_CONFIGURE_SMEM_ONCE(vq_bwd_wide_kernel, kVqWideBwdSmemMax);
+  vq_bwd_wide_kernel<<<blocks, kVqBwdThreads, vq_wide_bwd_smem_bytes(D), stream>>>(z, E, idx, g_out, g_loss, gz, gE, M, D, depth,
+                                                                                  residual, beta, use_norm);
+  B200_LAUNCH_OK("vq_bwd_wide_kernel");
   return 0;
 }
 
-// contributions [M * depth, 32], then the scatter's own scratch
+// contributions [M * depth, D], then the scatter's own scratch
 extern "C" size_t b200vq_vq_bwd_deterministic_workspace_bytes(int M, int K, int D, int depth) {
-  if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || D != kVqD) return 0;
+  if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || !vq_width_ok(D)) return 0;
   const long long n = (long long)M * depth;
-  const size_t contrib = ((size_t)n * kVqD * sizeof(float) + 255) & ~size_t(255);
-  return contrib + scatter_det_workspace_bytes(n, K, kVqD, kScatterRunVq);
+  const size_t contrib = ((size_t)n * D * sizeof(float) + 255) & ~size_t(255);
+  return contrib + scatter_det_workspace_bytes(n, K, D, kScatterRunVq);
 }
 
 extern "C" int b200vq_vq_bwd_deterministic(const float* z, const float* E, const long long* idx, const float* g_out,
                                            const float* g_loss, float* gz, float* gE, int M, int K, int D, int depth, int residual,
                                            float beta, int use_norm, void* workspace, size_t ws_bytes, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
   B200_CHECK_ARG(M > 0 && M % 4 == 0 && K > 0 && K % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
   B200_CHECK_ARG(z && E && idx && gz && gE && workspace, "vq_bwd_deterministic: null pointer argument");
   B200_CHECK_ARG(ws_bytes >= b200vq_vq_bwd_deterministic_workspace_bytes(M, K, D, depth), "vq_bwd_deterministic: workspace too small");
   const long long n = residual ? (long long)M * depth : M;   // entries: the plain quantiser reads idx[m]
   float* contrib = static_cast<float*>(workspace);
-  const size_t contrib_bytes = ((size_t)M * depth * kVqD * sizeof(float) + 255) & ~size_t(255);
-  vq_bwd_contrib_kernel<<<(M + 31) / 32, kVqBwdThreads, 0, stream>>>(z, E, idx, g_out, g_loss, gz, contrib, M, depth, residual,
-                                                                      beta, use_norm);
-  B200_LAUNCH_OK("vq_bwd_contrib_kernel");
-  return scatter_rows_det<kScatterRunVq>(idx, n, K, contrib, n, 0, 0, kVqD, gE, static_cast<uint8_t*>(workspace) + contrib_bytes,
+  const size_t contrib_bytes = ((size_t)M * depth * D * sizeof(float) + 255) & ~size_t(255);
+  if (D == kVqD) {
+    vq_bwd_contrib_kernel<<<(M + 31) / 32, kVqBwdThreads, 0, stream>>>(z, E, idx, g_out, g_loss, gz, contrib, M, depth, residual,
+                                                                        beta, use_norm);
+    B200_LAUNCH_OK("vq_bwd_contrib_kernel");
+  } else {
+    vq_bwd_contrib_wide_kernel<<<(M + kVqBwdThreads / 32 - 1) / (kVqBwdThreads / 32), kVqBwdThreads, 0, stream>>>(
+        z, E, idx, g_out, g_loss, gz, contrib, M, D, depth, residual, beta, use_norm);
+    B200_LAUNCH_OK("vq_bwd_contrib_wide_kernel");
+  }
+  return scatter_rows_det<kScatterRunVq>(idx, n, K, contrib, n, 0, 0, D, gE, static_cast<uint8_t*>(workspace) + contrib_bytes,
                                          ws_bytes - contrib_bytes, stream);
 }
 
 extern "C" int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
                                void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(D == kVqD, "vq: embed_dim must be %d", kVqD);
+  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
   B200_CHECK_ARG(M > 0 && M % 4 == 0 && depth >= 1, "vq_embed: bad sizes");
-  vq_embed_kernel<<<(M * 8 + 255) / 256, 256, 0, stream>>>(E, codes, out, M, K, depth, use_norm);
-  B200_LAUNCH_OK("vq_embed_kernel");
+  if (D == kVqD) {
+    vq_embed_kernel<<<(M * 8 + 255) / 256, 256, 0, stream>>>(E, codes, out, M, K, depth, use_norm);
+    B200_LAUNCH_OK("vq_embed_kernel");
+  } else {
+    vq_embed_wide_kernel<<<(M + 127) / 128, 128, 0, stream>>>(E, codes, out, M, K, D, depth, use_norm);
+    B200_LAUNCH_OK("vq_embed_wide_kernel");
+  }
   return 0;
 }
 
@@ -624,6 +1172,16 @@ __global__ void vq_ema_accumulate_kernel(const float* __restrict__ counts, const
   if (i >= K * kVqD) return;
   embed_avg[i] = decay * embed_avg[i] + one_minus_decay * sums[i];
   if (i % kVqD == 0) cluster_size[i / kVqD] = decay * cluster_size[i / kVqD] + one_minus_decay * counts[i / kVqD];
+}
+
+// vq_ema_accumulate_kernel at width D > 32
+__global__ void vq_ema_accumulate_wide_kernel(const float* __restrict__ counts, const float* __restrict__ sums,
+                                              float* __restrict__ cluster_size, float* __restrict__ embed_avg, int K, int D, float decay,
+                                              float one_minus_decay) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= K * D) return;
+  embed_avg[i] = decay * embed_avg[i] + one_minus_decay * sums[i];
+  if (i % D == 0) cluster_size[i / D] = decay * cluster_size[i / D] + one_minus_decay * counts[i / D];
 }
 
 // weight_k = embed_avg_k / ((cluster_size_k + eps) / (N + K eps) * N),  N = sum_k cluster_size_k.  Every CTA sums N itself
@@ -652,17 +1210,58 @@ vq_ema_weight_kernel(const float* __restrict__ cluster_size, const float* __rest
   }
 }
 
+// vq_ema_weight_kernel at width D > 32: the same N, the same fixed order
+__global__ void __launch_bounds__(256)
+vq_ema_weight_wide_kernel(const float* __restrict__ cluster_size, const float* __restrict__ embed_avg, float* __restrict__ weight, int K,
+                          int D, float eps, float k_eps) {
+  __shared__ float red[8];
+  float s = 0.f;
+  for (int k = threadIdx.x; k < K; k += 256) s += cluster_size[k];
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  float N = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) N += red[w];
+  const float denom = N + k_eps;
+  const int r0 = blockIdx.x * kVqEmaRowsPerCta;
+  for (int i = threadIdx.x; i < kVqEmaRowsPerCta * D; i += 256) {
+    const int k = r0 + i / D;
+    if (k >= K) break;
+    const float smoothed = (cluster_size[k] + eps) / denom * N;
+    weight[(size_t)k * D + i % D] = embed_avg[(size_t)k * D + i % D] / smoothed;
+  }
+}
+
 }  // namespace b200
 
-static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+// after the lookup: the EMA loss, the deterministic sums and the float counts
+static int vq_ema_finish(const long long* idx, float* loss, float* counts, float* sums, const int* icounts, const float* contrib,
+                         const float* part, int M, int K, int D, int depth, float beta, int deterministic, void* workspace,
+                         size_t ws_bytes, cudaStream_t stream) {
+  const long long n = (long long)M * depth;
+  const int nblk = (M + kVqTileM - 1) / kVqTileM;
+  vq_loss_kernel<true><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)D), beta, loss);
+  B200_LAUNCH_OK("vq_loss_kernel");
+  if (!counts) return 0;
+  if (deterministic) {
+    uint8_t* scratch = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(contrib)) + align256((size_t)n * D * sizeof(float));
+    const size_t used = (size_t)(scratch - static_cast<uint8_t*>(workspace));
+    const int rc = scatter_rows_det<kScatterRunVq>(idx, n, K, contrib, n, 0, 0, D, sums, scratch, ws_bytes - used, stream);
+    if (rc != 0) return rc;
+  }
+  vq_counts_to_float_kernel<<<(K + 255) / 256, 256, 0, stream>>>(icounts, counts, K);
+  B200_LAUNCH_OK("vq_counts_to_float_kernel");
+  return 0;
+}
 
-// [EnT | ee | loss parts] as b200vq_vq_fwd, [int counts K], deterministic: [contributions M*depth x 32 | scatter scratch]
+// [b200vq_vq_fwd's workspace], [int counts K], deterministic: [contributions M*depth x D | scatter scratch]
 extern "C" size_t b200vq_vq_fwd_ema_workspace_bytes(int M, int K, int D, int depth, int deterministic) {
-  if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || D != kVqD) return 0;
-  size_t b = align256(b200vq_vq_workspace_bytes(M, K, depth)) + align256((size_t)K * sizeof(int));
+  if (M <= 0 || K <= 0 || depth < 1 || depth > kVqMaxDepth || !vq_width_ok(D)) return 0;
+  size_t b = align256(b200vq_vq_fwd_workspace_bytes(M, K, D, depth)) + align256((size_t)K * sizeof(int));
   if (deterministic) {
     const long long n = (long long)M * depth;
-    b += align256((size_t)n * kVqD * sizeof(float)) + scatter_det_workspace_bytes(n, K, kVqD, kScatterRunVq);
+    b += align256((size_t)n * D * sizeof(float)) + scatter_det_workspace_bytes(n, K, D, kScatterRunVq);
   }
   return b;
 }
@@ -671,7 +1270,7 @@ extern "C" int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, lon
                                  int M, int K, int D, int depth, float beta, int use_norm, int deterministic, void* workspace,
                                  size_t ws_bytes, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(D == kVqD, "vq_fwd_ema: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(vq_width_ok(D), "vq_fwd_ema: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
   B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq_fwd_ema: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
   B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq_fwd_ema: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
   B200_CHECK_ARG(z && E && out && idx && loss && workspace, "vq_fwd_ema: null pointer argument");
@@ -682,13 +1281,23 @@ extern "C" int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, lon
   float* EnT = reinterpret_cast<float*>(ws);
   float* ee = EnT + (size_t)kVqD * K;
   float* part = ee + K;
-  ws += align256(b200vq_vq_workspace_bytes(M, K, depth));
+  ws += align256(b200vq_vq_fwd_workspace_bytes(M, K, D, depth));
   int* icounts = reinterpret_cast<int*>(ws);
   ws += align256((size_t)K * sizeof(int));
   float* contrib = reinterpret_cast<float*>(ws);
-  const long long n = (long long)M * depth;
   const int nblk = (M + kVqTileM - 1) / kVqTileM;
   const bool stats = counts != nullptr;
+  if (D != kVqD) {
+    if (stats) {
+      B200_CUDA_OK(cudaMemsetAsync(icounts, 0, (size_t)K * sizeof(int), stream));
+      if (!deterministic) B200_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)K * D * sizeof(float), stream));
+    }
+    const int mode = !stats ? kVqStatsOff : deterministic ? kVqStatsDeterministic : kVqStatsAtomic;
+    const int rc = vq_lookup_wide(z, E, out, idx, M, K, D, depth, use_norm, mode, icounts, sums, contrib, workspace, &part, stream);
+    if (rc != 0) return rc;
+    return vq_ema_finish(idx, loss, counts, sums, icounts, contrib, part, M, K, D, depth, beta, deterministic, workspace, ws_bytes,
+                         stream);
+  }
   vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
   B200_LAUNCH_OK("vq_prep_kernel");
   constexpr size_t stat_smem = kVqSmemBytes + sizeof(VqStatTable);
@@ -710,28 +1319,27 @@ extern "C" int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, lon
     }
   }
   B200_LAUNCH_OK("vq_fwd_kernel");
-  vq_loss_kernel<true><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)kVqD), beta, loss);
-  B200_LAUNCH_OK("vq_loss_kernel");
-  if (!stats) return 0;
-  if (deterministic) {
-    uint8_t* scratch = reinterpret_cast<uint8_t*>(contrib) + align256((size_t)n * kVqD * sizeof(float));
-    const size_t used = (size_t)(scratch - static_cast<uint8_t*>(workspace));
-    const int rc = scatter_rows_det<kScatterRunVq>(idx, n, K, contrib, n, 0, 0, kVqD, sums, scratch, ws_bytes - used, stream);
-    if (rc != 0) return rc;
-  }
-  vq_counts_to_float_kernel<<<(K + 255) / 256, 256, 0, stream>>>(icounts, counts, K);
-  B200_LAUNCH_OK("vq_counts_to_float_kernel");
-  return 0;
+  return vq_ema_finish(idx, loss, counts, sums, icounts, contrib, part, M, K, kVqD, depth, beta, deterministic, workspace, ws_bytes,
+                       stream);
 }
 
 extern "C" int b200vq_vq_ema_update(const float* counts, const float* sums, float* cluster_size, float* embed_avg, float* weight,
                                     int K, int D, float decay, float eps, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(D == kVqD, "vq_ema_update: embed_dim must be %d (got %d)", kVqD, D);
+  B200_CHECK_ARG(vq_width_ok(D), "vq_ema_update: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
   B200_CHECK_ARG(K > 0, "vq_ema_update: n_embed must be positive (got %d)", K);
   B200_CHECK_ARG(counts && sums && cluster_size && embed_avg && weight, "vq_ema_update: null pointer argument");
   B200_CHECK_ARG(decay >= 0.f && decay <= 1.f, "vq_ema_update: decay must be in [0, 1] (got %g)", (double)decay);
   B200_CHECK_ARG(eps >= 0.f, "vq_ema_update: eps must be non-negative (got %g)", (double)eps);
+  if (D != kVqD) {
+    vq_ema_accumulate_wide_kernel<<<(K * D + 255) / 256, 256, 0, stream>>>(counts, sums, cluster_size, embed_avg, K, D, decay,
+                                                                           (float)(1.0 - (double)decay));
+    B200_LAUNCH_OK("vq_ema_accumulate_wide_kernel");
+    vq_ema_weight_wide_kernel<<<(K + kVqEmaRowsPerCta - 1) / kVqEmaRowsPerCta, 256, 0, stream>>>(cluster_size, embed_avg, weight, K, D,
+                                                                                               eps, (float)((double)K * (double)eps));
+    B200_LAUNCH_OK("vq_ema_weight_wide_kernel");
+    return 0;
+  }
   vq_ema_accumulate_kernel<<<(K * kVqD + 255) / 256, 256, 0, stream>>>(counts, sums, cluster_size, embed_avg, K, decay,
                                                                        (float)(1.0 - (double)decay));
   B200_LAUNCH_OK("vq_ema_accumulate_kernel");

@@ -281,12 +281,13 @@ def attention_exact_bwd(qkv: Tensor, out: Tensor, lse: Tensor, dout: Tensor, B: 
 
 # ------------------------------------------------------------------------------------- quantiser
 def vq_fwd(z: Tensor, E: Tensor, depth: int, beta: float, use_norm: bool = True) -> Tuple[Tensor, Tensor, Tensor]:
-    """z [..., D], E [K, D] -> (straight-through value like z, loss scalar, idx int64 [M, depth])"""
+    """z [..., D], E [K, D] -> (straight-through value like z, loss scalar, idx int64 [M, depth]); D a multiple of 32
+    from 32 to 256"""
     _req(z, "z"); _req(E, "embedding.weight")
     K, D = E.shape
     M = z.numel() // D
     L = _lib.lib()
-    ws_bytes = L.b200vq_vq_workspace_bytes(M, K, depth)
+    ws_bytes = L.b200vq_vq_fwd_workspace_bytes(M, K, D, depth)
     ws = torch.empty(ws_bytes // 4, device=z.device, dtype=torch.float32)
     out = torch.empty_like(z)
     idx = torch.empty(M, depth, device=z.device, dtype=torch.int64)

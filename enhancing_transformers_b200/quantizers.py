@@ -8,7 +8,9 @@ residual mode the task calls "ResidualQuantizer" is ``use_residual=True, num_qua
 exactly as in the reference (there is no separate class there, SURVEY.md fact #1).
 
 Forward and backward each run as one fused CUDA launch sequence (csrc/vq.cu); the
-[tokens, n_embed] distance matrix of quantizers.py:78-80 is never materialised."""
+[tokens, n_embed] distance matrix of quantizers.py:78-80 is never materialised.  ``embed_dim`` may be any
+multiple of 32 from 32 to 256 (RQ-VAE quantises 256-wide features); other widths construct, as in the
+reference, and are rejected by the first forward."""
 from __future__ import annotations
 
 import math

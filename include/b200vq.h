@@ -127,8 +127,12 @@ int b200vq_attention_exact_bwd(const float* qkv, const float* out, const float* 
 /* ---- vector quantiser (quantizers.py:38-92) ------------------------------------------------------
  * z [M,D], codebook E [K,D] (un-normalised nn.Embedding weight); out [M,D] = straight-through
  * value z + (z_q - z); idx int64 [M, depth]; loss: device scalar.  depth = 1 for the plain
- * quantiser, num_quantizers for use_residual=True.  use_norm: quantizers.py:24 (1 = l2-normalise). */
+ * quantiser, num_quantizers for use_residual=True.  use_norm: quantizers.py:24 (1 = l2-normalise).
+ * Every VQ entry point takes embed_dim D = any multiple of 32 from 32 to 256 and rejects other widths.
+ * b200vq_vq_fwd_workspace_bytes: the forward workspace at width D (0 for an unsupported D); at D = 32 it equals
+ * b200vq_vq_workspace_bytes, the D = 32 query kept for existing callers. */
 size_t b200vq_vq_workspace_bytes(int M, int K, int depth);
+size_t b200vq_vq_fwd_workspace_bytes(int M, int K, int D, int depth);
 int b200vq_vq_fwd(const float* z, const float* E, float* out, long long* idx, float* loss, int M, int K, int D,
                   int depth, float beta, int use_norm, void* workspace, size_t ws_bytes, void* stream);
 /* g_out [M,D] or NULL, g_loss device scalar or NULL; gz [M,D] written, gE [K,D] zero-filled then
