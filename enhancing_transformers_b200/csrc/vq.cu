@@ -525,10 +525,13 @@ constexpr size_t kVqSmemBytes =
     sizeof(float4) * 8 * kVqThreads;
 
 // =============================================================================================
-// Wide codes: D = 32 * S for S in [2, 8] (D = 64 .. 256; RQ-VAE quantises 256-wide features).  The D = 32 kernels above
-// are not touched; the entry points pick these for D > 32.  Same arithmetic contract: distances fmaf(-2, dot, |z|^2 +
-// |e|^2) with dot summed by fmaf in ascending k, lowest index among equal distances, straight-through z + (acc - z),
-// normalisation by true division by max(|x|, 1e-12).
+// Wide codes: D = 32 * S for S in [2, 8] (D = 64 .. 256; RQ-VAE quantises 256-wide features).  The entry points pick these
+// kernels for D > 32 through one host path (vq_lookup), and the EMA update kernels below serve every width.  The D = 32
+// kernels above stay separate: the two families normalise in different summation orders (each vq_embed must equal its
+// own lookup bit for bit), and running the D = 32 lookup on this kernel's phase B and statistics pass measured slower
+// (DESIGN.md §7.6).  Same arithmetic contract: distances fmaf(-2, dot, |z|^2 + |e|^2) with dot summed by fmaf in
+// ascending k, lowest index among equal distances, straight-through z + (acc - z), normalisation by true division by
+// max(|x|, 1e-12).
 //   - A row's squared norm is one thread's fmaf chain in column order (vq_row_sq): the lookup's phase A, its gather,
 //     vq_prep and vq_embed all normalise a row with the same bits, so vq_embed equals the lookup's accumulated code.
 //   - The lookup keeps the whole normalised tile zT [D][128] in shared memory and streams E^T through a two-stage ring
@@ -1008,76 +1011,100 @@ __global__ void vq_embed_wide_kernel(const float* __restrict__ E, const long lon
 
 using namespace b200;
 
-extern "C" size_t b200vq_vq_workspace_bytes(int M, int K, int depth) {
-  const size_t nblk = (M + kVqTileM - 1) / kVqTileM;
-  return ((size_t)kVqD * K + K + (size_t)depth * nblk) * sizeof(float);
-}
-
 static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 
-extern "C" size_t b200vq_vq_fwd_workspace_bytes(int M, int K, int D, int depth) {
-  if (!vq_width_ok(D)) return 0;
-  if (D == kVqD) return b200vq_vq_workspace_bytes(M, K, depth);
-  // [EnT D x K | ee K | loss parts depth x blocks], then the raw residual [M, D] of the depth loop
+// The lookup's workspace, byte offsets: [EnT D x K | ee K | loss parts depth x blocks], then for D > 32 at depth > 1 the
+// raw residual [M, D] of the depth loop (rws == 0: none)
+struct VqFwdLayout {
+  size_t ee, part, rws, bytes;
+};
+static VqFwdLayout vq_fwd_layout(int M, int K, int D, int depth) {
   const size_t nblk = (M + kVqTileM - 1) / kVqTileM;
-  const size_t base = ((size_t)D * K + K + (size_t)depth * nblk) * sizeof(float);
-  return depth > 1 ? align256(base) + (size_t)M * D * sizeof(float) : base;
+  VqFwdLayout l;
+  l.ee = (size_t)D * K * sizeof(float);
+  l.part = l.ee + (size_t)K * sizeof(float);
+  l.bytes = l.part + (size_t)depth * nblk * sizeof(float);
+  l.rws = 0;
+  if (D > kVqD && depth > 1) {
+    l.rws = align256(l.bytes);
+    l.bytes = l.rws + (size_t)M * D * sizeof(float);
+  }
+  return l;
 }
 
-// vq_prep + the lookup at D > 32 into the b200vq_vq_fwd_workspace_bytes layout; part receives the loss partial sums
-static int vq_lookup_wide(const float* z, const float* E, float* out, long long* idx, int M, int K, int D, int depth, int use_norm,
-                          int stats, int* icounts, float* sums, float* contrib, void* workspace, float** part, cudaStream_t stream) {
-  float* EnT = static_cast<float*>(workspace);
-  float* ee = EnT + (size_t)D * K;
-  *part = ee + K;
-  const int nblk = (M + kVqTileM - 1) / kVqTileM;
-  float* rws = depth > 1 ? reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) +
-                                                     align256(((size_t)D * K + K + (size_t)depth * nblk) * sizeof(float)))
-                         : nullptr;
-  vq_prep_wide_kernel<<<(K + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, D, use_norm);
-  B200_LAUNCH_OK("vq_prep_wide_kernel");
-  const size_t smem = vq_wide_smem_bytes(D, stats != kVqStatsOff);
-  if (stats == kVqStatsOff) {
-    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kVqStatsOff>, vq_wide_smem_bytes(kVqMaxD, false));
-    vq_fwd_wide_kernel<kVqStatsOff><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth,
-                                                                        use_norm, nullptr, nullptr, nullptr);
-  } else if (stats == kVqStatsAtomic) {
-    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kVqStatsAtomic>, vq_wide_smem_bytes(kVqMaxD, true));
-    vq_fwd_wide_kernel<kVqStatsAtomic><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth,
-                                                                           use_norm, icounts, sums, nullptr);
-  } else {
-    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kVqStatsDeterministic>, vq_wide_smem_bytes(kVqMaxD, true));
-    vq_fwd_wide_kernel<kVqStatsDeterministic><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, rws, idx, *part, M, K, D,
-                                                                                  depth, use_norm, icounts, nullptr, contrib);
-  }
-  B200_LAUNCH_OK("vq_fwd_wide_kernel");
+extern "C" size_t b200vq_vq_workspace_bytes(int M, int K, int depth) { return vq_fwd_layout(M, K, kVqD, depth).bytes; }
+
+extern "C" size_t b200vq_vq_fwd_workspace_bytes(int M, int K, int D, int depth) {
+  return vq_width_ok(D) ? vq_fwd_layout(M, K, D, depth).bytes : 0;
+}
+
+// The shape checks of the quantiser's entry points, in this order: width, sizes, depth.  `who` prefixes the messages.
+static int vq_check_shapes(const char* who, int M, int K, int D, int depth) {
+  B200_CHECK_ARG(vq_width_ok(D), "%s: embed_dim must be a multiple of 32 in [32, 256] (got %d)", who, D);
+  B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "%s: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", who, M, K);
+  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "%s: num_quantizers must be in [1,%d] (got %d)", who, kVqMaxDepth, depth);
   return 0;
+}
+
+template <int kStats>
+static int vq_launch_lookup(const float* z, const float* EnT, const float* ee, const float* E, float* out, float* rws, long long* idx,
+                            float* part, int M, int K, int D, int depth, int use_norm, int* icounts, float* sums, float* contrib,
+                            cudaStream_t stream) {
+  constexpr bool stats = kStats != kVqStatsOff;
+  const int nblk = (M + kVqTileM - 1) / kVqTileM;
+  if (D == kVqD) {
+    constexpr size_t smem = kVqSmemBytes + (stats ? sizeof(VqStatTable) : 0);
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kStats>, smem);
+    vq_fwd_kernel<kStats><<<nblk, kVqThreads, smem, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm, icounts, sums,
+                                                              contrib);
+    B200_LAUNCH_OK("vq_fwd_kernel");
+  } else {
+    B200_CONFIGURE_SMEM_ONCE(vq_fwd_wide_kernel<kStats>, vq_wide_smem_bytes(kVqMaxD, stats));
+    vq_fwd_wide_kernel<kStats><<<nblk, kVqThreads, vq_wide_smem_bytes(D, stats), stream>>>(z, EnT, ee, E, out, rws, idx, part, M, K,
+                                                                                           D, depth, use_norm, icounts, sums,
+                                                                                           contrib);
+    B200_LAUNCH_OK("vq_fwd_wide_kernel");
+  }
+  return 0;
+}
+
+// vq_prep + the lookup at any width and in any statistics mode, in the vq_fwd_layout workspace; *part receives the loss
+// partial sums
+static int vq_lookup(const float* z, const float* E, float* out, long long* idx, int M, int K, int D, int depth, int use_norm,
+                     int stats, int* icounts, float* sums, float* contrib, void* workspace, float** part, cudaStream_t stream) {
+  const VqFwdLayout l = vq_fwd_layout(M, K, D, depth);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  float* EnT = reinterpret_cast<float*>(ws);
+  float* ee = reinterpret_cast<float*>(ws + l.ee);
+  float* rws = l.rws ? reinterpret_cast<float*>(ws + l.rws) : nullptr;
+  *part = reinterpret_cast<float*>(ws + l.part);
+  if (D == kVqD) {
+    vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
+    B200_LAUNCH_OK("vq_prep_kernel");
+  } else {
+    vq_prep_wide_kernel<<<(K + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, D, use_norm);
+    B200_LAUNCH_OK("vq_prep_wide_kernel");
+  }
+  if (stats == kVqStatsOff)
+    return vq_launch_lookup<kVqStatsOff>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth, use_norm, icounts, sums, contrib,
+                                         stream);
+  if (stats == kVqStatsAtomic)
+    return vq_launch_lookup<kVqStatsAtomic>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth, use_norm, icounts, sums, contrib,
+                                            stream);
+  return vq_launch_lookup<kVqStatsDeterministic>(z, EnT, ee, E, out, rws, idx, *part, M, K, D, depth, use_norm, icounts, sums, contrib,
+                                                 stream);
 }
 
 extern "C" int b200vq_vq_fwd(const float* z, const float* E, float* out, long long* idx, float* loss, int M, int K, int D, int depth,
                              float beta, int use_norm, void* workspace, size_t ws_bytes, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
-  B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
-  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d]", kVqMaxDepth);
+  if (const int rc = vq_check_shapes("vq", M, K, D, depth)) return rc;
   B200_CHECK_ARG(ws_bytes >= b200vq_vq_fwd_workspace_bytes(M, K, D, depth), "vq: workspace too small");
-  const int nblk = (M + kVqTileM - 1) / kVqTileM;
   float* part;
-  if (D == kVqD) {
-    float* EnT = static_cast<float*>(workspace);
-    float* ee = EnT + (size_t)kVqD * K;
-    part = ee + K;
-    vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
-    B200_LAUNCH_OK("vq_prep_kernel");
-    B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsOff>, kVqSmemBytes);
-    vq_fwd_kernel<kVqStatsOff><<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
-                                                                           nullptr, nullptr, nullptr);
-    B200_LAUNCH_OK("vq_fwd_kernel");
-  } else {
-    const int rc = vq_lookup_wide(z, E, out, idx, M, K, D, depth, use_norm, kVqStatsOff, nullptr, nullptr, nullptr, workspace, &part,
-                                  stream);
-    if (rc != 0) return rc;
-  }
+  if (const int rc = vq_lookup(z, E, out, idx, M, K, D, depth, use_norm, kVqStatsOff, nullptr, nullptr, nullptr, workspace, &part,
+                               stream))
+    return rc;
+  const int nblk = (M + kVqTileM - 1) / kVqTileM;
   vq_loss_kernel<false><<<1, 256, 0, stream>>>(part, nblk, depth, 1.f / ((float)M * (float)D), beta, loss);
   B200_LAUNCH_OK("vq_loss_kernel");
   return 0;
@@ -1086,9 +1113,7 @@ extern "C" int b200vq_vq_fwd(const float* z, const float* E, float* out, long lo
 extern "C" int b200vq_vq_bwd(const float* z, const float* E, const long long* idx, const float* g_out, const float* g_loss, float* gz,
                              float* gE, int M, int K, int D, int depth, int residual, float beta, int use_norm, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
-  B200_CHECK_ARG(M > 0 && M % 4 == 0, "vq: need M %% 4 == 0");
-  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: bad depth");
+  if (const int rc = vq_check_shapes("vq", M, K, D, depth)) return rc;
   B200_CUDA_OK(cudaMemsetAsync(gE, 0, (size_t)K * D * sizeof(float), stream));
   const int cap = num_sms() * 2;          // few, long-lived CTAs: each aggregates ~M / cap tokens in its table
   if (D == kVqD) {
@@ -1119,9 +1144,7 @@ extern "C" int b200vq_vq_bwd_deterministic(const float* z, const float* E, const
                                            const float* g_loss, float* gz, float* gE, int M, int K, int D, int depth, int residual,
                                            float beta, int use_norm, void* workspace, size_t ws_bytes, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
-  B200_CHECK_ARG(M > 0 && M % 4 == 0 && K > 0 && K % 4 == 0, "vq: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
-  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
+  if (const int rc = vq_check_shapes("vq", M, K, D, depth)) return rc;
   B200_CHECK_ARG(z && E && idx && gz && gE && workspace, "vq_bwd_deterministic: null pointer argument");
   B200_CHECK_ARG(ws_bytes >= b200vq_vq_bwd_deterministic_workspace_bytes(M, K, D, depth), "vq_bwd_deterministic: workspace too small");
   const long long n = residual ? (long long)M * depth : M;   // entries: the plain quantiser reads idx[m]
@@ -1143,8 +1166,7 @@ extern "C" int b200vq_vq_bwd_deterministic(const float* z, const float* E, const
 extern "C" int b200vq_vq_embed(const float* E, const long long* codes, float* out, int M, int K, int D, int depth, int use_norm,
                                void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(vq_width_ok(D), "vq: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
-  B200_CHECK_ARG(M > 0 && M % 4 == 0 && depth >= 1, "vq_embed: bad sizes");
+  if (const int rc = vq_check_shapes("vq_embed", M, K, D, depth)) return rc;
   if (D == kVqD) {
     vq_embed_kernel<<<(M * 8 + 255) / 256, 256, 0, stream>>>(E, codes, out, M, K, depth, use_norm);
     B200_LAUNCH_OK("vq_embed_kernel");
@@ -1164,17 +1186,7 @@ __global__ void vq_counts_to_float_kernel(const int* __restrict__ icounts, float
   if (k < K) counts[k] = (float)icounts[k];    // exact: a count never exceeds M * depth < 2^24 (checked by the host)
 }
 
-// cluster_size <- decay * cluster_size + (1 - decay) * n;  embed_avg <- decay * embed_avg + (1 - decay) * s
-__global__ void vq_ema_accumulate_kernel(const float* __restrict__ counts, const float* __restrict__ sums,
-                                         float* __restrict__ cluster_size, float* __restrict__ embed_avg, int K, float decay,
-                                         float one_minus_decay) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= K * kVqD) return;
-  embed_avg[i] = decay * embed_avg[i] + one_minus_decay * sums[i];
-  if (i % kVqD == 0) cluster_size[i / kVqD] = decay * cluster_size[i / kVqD] + one_minus_decay * counts[i / kVqD];
-}
-
-// vq_ema_accumulate_kernel at width D > 32
+// cluster_size <- decay * cluster_size + (1 - decay) * n;  embed_avg <- decay * embed_avg + (1 - decay) * s  (any width D)
 __global__ void vq_ema_accumulate_wide_kernel(const float* __restrict__ counts, const float* __restrict__ sums,
                                               float* __restrict__ cluster_size, float* __restrict__ embed_avg, int K, int D, float decay,
                                               float one_minus_decay) {
@@ -1188,29 +1200,6 @@ __global__ void vq_ema_accumulate_wide_kernel(const float* __restrict__ counts, 
 // in the same fixed order (strided per thread, then the warps' partials in order), so N has the same bits in every CTA
 // and on every run, and no grid-wide barrier or scratch is needed.
 constexpr int kVqEmaRowsPerCta = 64;
-__global__ void __launch_bounds__(256)
-vq_ema_weight_kernel(const float* __restrict__ cluster_size, const float* __restrict__ embed_avg, float* __restrict__ weight, int K,
-                     float eps, float k_eps) {
-  __shared__ float red[8];
-  float s = 0.f;
-  for (int k = threadIdx.x; k < K; k += 256) s += cluster_size[k];
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  float N = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) N += red[w];
-  const float denom = N + k_eps;
-  const int r0 = blockIdx.x * kVqEmaRowsPerCta;
-  for (int i = threadIdx.x; i < kVqEmaRowsPerCta * kVqD; i += 256) {
-    const int k = r0 + i / kVqD;
-    if (k >= K) break;
-    const float smoothed = (cluster_size[k] + eps) / denom * N;
-    weight[(size_t)k * kVqD + i % kVqD] = embed_avg[(size_t)k * kVqD + i % kVqD] / smoothed;
-  }
-}
-
-// vq_ema_weight_kernel at width D > 32: the same N, the same fixed order
 __global__ void __launch_bounds__(256)
 vq_ema_weight_wide_kernel(const float* __restrict__ cluster_size, const float* __restrict__ embed_avg, float* __restrict__ weight, int K,
                           int D, float eps, float k_eps) {
@@ -1270,56 +1259,24 @@ extern "C" int b200vq_vq_fwd_ema(const float* z, const float* E, float* out, lon
                                  int M, int K, int D, int depth, float beta, int use_norm, int deterministic, void* workspace,
                                  size_t ws_bytes, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(vq_width_ok(D), "vq_fwd_ema: embed_dim must be a multiple of 32 in [32, 256] (got %d)", D);
-  B200_CHECK_ARG(M > 0 && K > 0 && K % 4 == 0 && M % 4 == 0, "vq_fwd_ema: need M %% 4 == 0 and n_embed %% 4 == 0 (M=%d K=%d)", M, K);
-  B200_CHECK_ARG(depth >= 1 && depth <= kVqMaxDepth, "vq_fwd_ema: num_quantizers must be in [1,%d] (got %d)", kVqMaxDepth, depth);
+  if (const int rc = vq_check_shapes("vq_fwd_ema", M, K, D, depth)) return rc;
   B200_CHECK_ARG(z && E && out && idx && loss && workspace, "vq_fwd_ema: null pointer argument");
   B200_CHECK_ARG((counts == nullptr) == (sums == nullptr), "vq_fwd_ema: counts and sums must both be given or both be NULL");
   B200_CHECK_ARG((long long)M * depth < (1ll << 24), "vq_fwd_ema: M * depth must be below 2^24 (fp32 counts stay exact)");
   B200_CHECK_ARG(ws_bytes >= b200vq_vq_fwd_ema_workspace_bytes(M, K, D, depth, deterministic), "vq_fwd_ema: workspace too small");
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  float* EnT = reinterpret_cast<float*>(ws);
-  float* ee = EnT + (size_t)kVqD * K;
-  float* part = ee + K;
-  ws += align256(b200vq_vq_fwd_workspace_bytes(M, K, D, depth));
+  uint8_t* ws = static_cast<uint8_t*>(workspace) + align256(b200vq_vq_fwd_workspace_bytes(M, K, D, depth));
   int* icounts = reinterpret_cast<int*>(ws);
-  ws += align256((size_t)K * sizeof(int));
-  float* contrib = reinterpret_cast<float*>(ws);
-  const int nblk = (M + kVqTileM - 1) / kVqTileM;
+  float* contrib = reinterpret_cast<float*>(ws + align256((size_t)K * sizeof(int)));
   const bool stats = counts != nullptr;
-  if (D != kVqD) {
-    if (stats) {
-      B200_CUDA_OK(cudaMemsetAsync(icounts, 0, (size_t)K * sizeof(int), stream));
-      if (!deterministic) B200_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)K * D * sizeof(float), stream));
-    }
-    const int mode = !stats ? kVqStatsOff : deterministic ? kVqStatsDeterministic : kVqStatsAtomic;
-    const int rc = vq_lookup_wide(z, E, out, idx, M, K, D, depth, use_norm, mode, icounts, sums, contrib, workspace, &part, stream);
-    if (rc != 0) return rc;
-    return vq_ema_finish(idx, loss, counts, sums, icounts, contrib, part, M, K, D, depth, beta, deterministic, workspace, ws_bytes,
-                         stream);
-  }
-  vq_prep_kernel<<<(K * 8 + 255) / 256, 256, 0, stream>>>(E, EnT, ee, K, use_norm);
-  B200_LAUNCH_OK("vq_prep_kernel");
-  constexpr size_t stat_smem = kVqSmemBytes + sizeof(VqStatTable);
-  if (!stats) {
-    B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsOff>, kVqSmemBytes);
-    vq_fwd_kernel<kVqStatsOff><<<nblk, kVqThreads, kVqSmemBytes, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
-                                                                           nullptr, nullptr, nullptr);
-  } else {
+  if (stats) {
     B200_CUDA_OK(cudaMemsetAsync(icounts, 0, (size_t)K * sizeof(int), stream));
-    if (deterministic) {
-      B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsDeterministic>, stat_smem);
-      vq_fwd_kernel<kVqStatsDeterministic><<<nblk, kVqThreads, stat_smem, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth,
-                                                                                    use_norm, icounts, nullptr, contrib);
-    } else {
-      B200_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)K * kVqD * sizeof(float), stream));
-      B200_CONFIGURE_SMEM_ONCE(vq_fwd_kernel<kVqStatsAtomic>, stat_smem);
-      vq_fwd_kernel<kVqStatsAtomic><<<nblk, kVqThreads, stat_smem, stream>>>(z, EnT, ee, E, out, idx, part, M, K, depth, use_norm,
-                                                                             icounts, sums, nullptr);
-    }
+    if (!deterministic) B200_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)K * D * sizeof(float), stream));
   }
-  B200_LAUNCH_OK("vq_fwd_kernel");
-  return vq_ema_finish(idx, loss, counts, sums, icounts, contrib, part, M, K, kVqD, depth, beta, deterministic, workspace, ws_bytes,
+  const int mode = !stats ? kVqStatsOff : deterministic ? kVqStatsDeterministic : kVqStatsAtomic;
+  float* part;
+  if (const int rc = vq_lookup(z, E, out, idx, M, K, D, depth, use_norm, mode, icounts, sums, contrib, workspace, &part, stream))
+    return rc;
+  return vq_ema_finish(idx, loss, counts, sums, icounts, contrib, part, M, K, D, depth, beta, deterministic, workspace, ws_bytes,
                        stream);
 }
 
@@ -1331,20 +1288,11 @@ extern "C" int b200vq_vq_ema_update(const float* counts, const float* sums, floa
   B200_CHECK_ARG(counts && sums && cluster_size && embed_avg && weight, "vq_ema_update: null pointer argument");
   B200_CHECK_ARG(decay >= 0.f && decay <= 1.f, "vq_ema_update: decay must be in [0, 1] (got %g)", (double)decay);
   B200_CHECK_ARG(eps >= 0.f, "vq_ema_update: eps must be non-negative (got %g)", (double)eps);
-  if (D != kVqD) {
-    vq_ema_accumulate_wide_kernel<<<(K * D + 255) / 256, 256, 0, stream>>>(counts, sums, cluster_size, embed_avg, K, D, decay,
-                                                                           (float)(1.0 - (double)decay));
-    B200_LAUNCH_OK("vq_ema_accumulate_wide_kernel");
-    vq_ema_weight_wide_kernel<<<(K + kVqEmaRowsPerCta - 1) / kVqEmaRowsPerCta, 256, 0, stream>>>(cluster_size, embed_avg, weight, K, D,
-                                                                                               eps, (float)((double)K * (double)eps));
-    B200_LAUNCH_OK("vq_ema_weight_wide_kernel");
-    return 0;
-  }
-  vq_ema_accumulate_kernel<<<(K * kVqD + 255) / 256, 256, 0, stream>>>(counts, sums, cluster_size, embed_avg, K, decay,
-                                                                       (float)(1.0 - (double)decay));
-  B200_LAUNCH_OK("vq_ema_accumulate_kernel");
-  vq_ema_weight_kernel<<<(K + kVqEmaRowsPerCta - 1) / kVqEmaRowsPerCta, 256, 0, stream>>>(cluster_size, embed_avg, weight, K, eps,
-                                                                                        (float)((double)K * (double)eps));
-  B200_LAUNCH_OK("vq_ema_weight_kernel");
+  vq_ema_accumulate_wide_kernel<<<(K * D + 255) / 256, 256, 0, stream>>>(counts, sums, cluster_size, embed_avg, K, D, decay,
+                                                                         (float)(1.0 - (double)decay));
+  B200_LAUNCH_OK("vq_ema_accumulate_wide_kernel");
+  vq_ema_weight_wide_kernel<<<(K + kVqEmaRowsPerCta - 1) / kVqEmaRowsPerCta, 256, 0, stream>>>(cluster_size, embed_avg, weight, K, D,
+                                                                                             eps, (float)((double)K * (double)eps));
+  B200_LAUNCH_OK("vq_ema_weight_wide_kernel");
   return 0;
 }
