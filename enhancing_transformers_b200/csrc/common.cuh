@@ -69,10 +69,15 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 // symbol: a round trip through uintptr_t loses the address space and every later access becomes a generic LD / ST.
 __device__ __forceinline__ uint8_t* smem_align1024(uint8_t* raw) { return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u); }
 // round-to-nearest (ties away from zero, like cvt.rna.tf32.f32) fp32 -> tf32 (10-bit mantissa),
-// result kept in an fp32 container with the low 13 bits cleared.  Two integer ops on the ALU pipe
-// instead of cvt.rna.tf32, which issues on the XU pipe shared with ex2.
+// result kept in an fp32 container with the low 13 bits cleared.  Integer ops on the ALU pipe
+// instead of cvt.rna.tf32, which issues on the XU pipe shared with ex2.  A NaN keeps its sign and gets
+// the quiet bit instead of the rounding carry: the carry would run out of the mantissa (0x7FFFFFFF, the
+// NaN every fp32 operation on the GPU makes, would become -0.0), and the quiet bit survives the tensor
+// core's truncation.  Finite values and +-inf round as before.
 __device__ __forceinline__ float round_tf32(float x) {
-  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+  const uint32_t u = __float_as_uint(x);
+  const bool nan = (u & 0x7FFFFFFFu) > 0x7F800000u;
+  return __uint_as_float((nan ? (u | 0x00400000u) : (u + 0x1000u)) & 0xFFFFE000u);
 }
 // tanh(x) = 1 - 2 / (exp(2x) + 1) with one ex2.approx and one rcp.approx (absolute error ~1e-7, far below the
 // tf32 rounding applied to the result).  libdevice's tanhf costs ~40 instructions per element of the MLP-1 epilogue.

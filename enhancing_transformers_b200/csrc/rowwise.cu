@@ -375,7 +375,8 @@ __global__ void grad_scale_kernel(const unsigned* __restrict__ part, int nparts,
     float S = 1.f;
     if (amax > 0.f && amax < INFINITY) {          // zero / inf / nan gradients: leave unscaled
       int e;
-      frexpf(amax, &e);                          // amax = f * 2^e, f in [0.5, 1)  ->  amax <= 2^e
+      const float f = frexpf(amax, &e);          // amax = f * 2^e, f in [0.5, 1)  ->  amax <= 2^e
+      if (f == 0.5f) --e;                        // amax = 2^(e-1) exactly: ceil(log2(amax)) = e - 1
       int sh = target_log2 - e;
       sh = sh > 100 ? 100 : (sh < -100 ? -100 : sh);
       S = ldexpf(1.f, sh);

@@ -74,12 +74,15 @@ time_mix_bwd_kernel(const float* __restrict__ g, const float* __restrict__ x, co
   reinterpret_cast<float4*>(gw_part)[(long long)blockIdx.y * C4 + c] = acc;
 }
 
+// torch.relu's threshold rule, x <= 0 ? 0 : x: NaN passes through (fmaxf(NaN, 0) would give 0) and -0 becomes +0
+__device__ __forceinline__ float relu_nan(float v) { return v <= 0.f ? 0.f : v; }
+
 // grad 0: y = relu(x)^2 ; grad 1: y = g * 2 * relu(x)   (x = the pre-activation in both cases)
 __global__ void __launch_bounds__(256)
 sqrelu_kernel(const float* __restrict__ x, const float* __restrict__ g, float* __restrict__ y, long long n4, int grad, int round_out) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const float4 v = reinterpret_cast<const float4*>(x)[i];
-    const float4 r = make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f));
+    const float4 r = make_float4(relu_nan(v.x), relu_nan(v.y), relu_nan(v.z), relu_nan(v.w));
     float4 o;
     if (grad) {
       const float4 gv = reinterpret_cast<const float4*>(g)[i];

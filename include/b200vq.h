@@ -178,7 +178,10 @@ int b200vq_unpatchify(const float* tokens, const float* bias, float* img, int B,
 size_t b200vq_colsum_workspace_bytes(int N);
 /* out[n] = sum_m X[m,n] (bias gradients) */
 int b200vq_colsum(const float* X, long long ld, int M, int N, float* out, void* workspace, size_t ws_bytes, void* stream);
-/* out = tf32-rounded copy of in (weights shadow for the tensor-core path) */
+/* out = tf32-rounded copy of in (weights shadow for the tensor-core path): round to nearest, ties away from zero, as
+ * cvt.rna.tf32.f32 does, kept in an fp32 container with the low 13 bits clear (values past the largest tf32 become
+ * inf).  NaN stays NaN with its sign: the quiet bit is set, so it is still NaN after a tensor core truncates it.  Every
+ * round_out of this header rounds the same way. */
 int b200vq_round_tf32(const float* in, float* out, long long n, void* stream);
 
 /* out[m,:] = x[m,:] + table[m % R,:]  (token + de_pos_embedding, layers.py:210) */
@@ -191,7 +194,9 @@ int b200vq_split_tf32_lo(const float* in, float* lo, long long n, void* stream);
 /* out16 = fp16(in * *scale), saturating at +-65504 (scale: device scalar or NULL) */
 int b200vq_to_half(const float* in, void* out16, long long n, const float* scale, void* stream);
 /* scale2 = {S, 1/S}, S = 2^(target_log2 - ceil(log2(max|g|))): the power-of-two gradient scale of one backward
- * segment, chosen on the device from the incoming gradient (no host synchronisation) */
+ * segment, chosen on the device from the incoming gradient (no host synchronisation), so max|g| * S lies in
+ * (2^(target_log2-1), 2^target_log2].  The exponent is clamped to [-100, 100] (a subnormal or huge max|g|), and a
+ * gradient whose max|g| is zero, inf or NaN gets S = 1. */
 size_t b200vq_grad_scale_workspace_bytes(void);
 int b200vq_grad_scale(const float* g, long long n, int target_log2, float* scale2, void* workspace, size_t ws_bytes,
                       void* stream);
