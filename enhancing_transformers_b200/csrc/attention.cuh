@@ -23,5 +23,12 @@ int attention_exact_forward(const float* qkv, float* out, float* lse, int B, int
                             int cond_len, cudaStream_t stream);
 int attention_exact_backward(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv, float* delta,
                              int B, int N, int heads, int dh, float scale, int cond_len, cudaStream_t stream);
+// Wide heads (dh 96 / 128), stage-2 mask only (cond_len >= 0), fp32 in and out: exact != 0 -> 3xTF32, otherwise one tf32
+// pass with round_out.  The backward computes delta itself.
+int attention_wide_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale, int cond_len,
+                           int exact, int round_out, cudaStream_t stream);
+int attention_wide_backward(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv, float* delta,
+                            int B, int N, int heads, int dh, float scale, int cond_len, int exact, int round_out,
+                            cudaStream_t stream);
 
 }  // namespace b200

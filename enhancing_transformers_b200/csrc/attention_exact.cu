@@ -458,6 +458,400 @@ attn_bwd_dq_kernel(const void* __restrict__ qkv_, const void* __restrict__ dout_
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Wide heads (DH 96 / 128, stage-2 mask, fp32 in and out).  At these widths a warp's resident operand fragments
+// (DH/2 registers each) no longer fit next to its accumulators, so the resident operand of each kernel (forward: Q;
+// key side: K, V; query side: Q, dO) is staged once in shared memory and its A fragments are read per k-step, the
+// way the streamed tiles' B fragments are.  Registers then hold only the DH/8 x 4 accumulators and the score tiles.
+// Every kernel is 8 warps x 16 resident rows = 128 rows per CTA; the streamed tiles are double-buffered, KB rows each
+// (forward 64; backward 32, which keeps the score, dP and dS tiles of the key side at 16 registers each beside the
+// 2 x DH/2 registers of dK and dV).  Shared memory at DH 128: 384 padded rows of 528 bytes = 198 KB per CTA.
+// ---------------------------------------------------------------------------------------------
+constexpr int kWideRows = 128;   // resident rows per CTA (8 warps x 16)
+
+// A fragment (k-step k) of the warp's 16-row block `As` of a staged tile (row pitch Pitch::LDS)
+template <int DH>
+__device__ __forceinline__ void lds_a_frag(uint32_t (&a)[4], const float* As, int k, int lane) {
+  constexpr int LDS = Pitch<float, DH>::LDS;
+  const float* p = As + (lane >> 2) * LDS + k * 8 + (lane & 3);
+  a[0] = ldbits(p); a[1] = ldbits(p + 8 * LDS); a[2] = ldbits(p + 4); a[3] = ldbits(p + 8 * LDS + 4);
+}
+// acc[nt] (16 x 8 each, NT column tiles) += A(16 x DH, staged rows As) . T^T, T a staged tile whose rows are the output
+// columns (mma_rows_x_tileT with the A operand from shared memory)
+template <int DH, int PASSES, int NT>
+__device__ __forceinline__ void mma_srows_x_tileT(float (&acc)[NT][4], const float* As, const float* Ts, int lane) {
+  constexpr int LDS = Pitch<float, DH>::LDS;
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int k = 0; k < DH / 8; ++k) {
+    uint32_t a[4];
+    lds_a_frag<DH>(a, As, k, lane);
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      const float* p = Ts + (nt * 8 + g) * LDS + k * 8 + t;
+      mma_x<PASSES>(acc[nt], a, ldbits(p), ldbits(p + 4));
+    }
+  }
+}
+// acc[dt] += P(16 x 8 NT, accumulator-layout fragments) . T, T a staged tile whose rows are the contraction index
+// (mma_p_x_tile over NT k-steps)
+template <int DH, int PASSES, int NT>
+__device__ __forceinline__ void mma_pn_x_tile(float (&acc)[DH / 8][4], const uint32_t (&p)[NT][4], const float* Ts, int lane) {
+  constexpr int LDS = Pitch<float, DH>::LDS;
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int kt = 0; kt < NT; ++kt)
+#pragma unroll
+    for (int dt = 0; dt < DH / 8; ++dt) {
+      const float* q = Ts + (kt * 8 + 2 * t) * LDS + dt * 8 + g;
+      mma_x<PASSES>(acc[dt], p[kt], ldbits(q), ldbits(q + LDS));
+    }
+}
+
+// forward: grid (ceil(N/128), heads, B); Q[128 rows], K[2][64 rows], V[2][64 rows]
+template <int DH, int PASSES>
+__global__ void __launch_bounds__(256, 1)
+attn_fwd_wide_kernel(const float* __restrict__ qkv, float* __restrict__ out, float* __restrict__ lse, int N, int heads, float scale,
+                     int cond, int round_out) {
+  constexpr int LDS = Pitch<float, DH>::LDS;
+  constexpr int KB = 64, NT = KB / 8;
+  constexpr int TILE = KB * LDS;
+  extern __shared__ __align__(16) uint8_t sm_raw[];
+  float* Qs = reinterpret_cast<float*>(sm_raw);
+  float* Ks = Qs + kWideRows * LDS;
+  float* Vs = Ks + 2 * TILE;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int inner = heads * DH;
+  const long long ld = 3ll * inner;
+  const float* qbase = qkv + (long long)b * N * ld + h * DH;
+  const float* kbase = qbase + inner;
+  const float* vbase = qbase + 2 * inner;
+  const int qb = blockIdx.x * kWideRows;
+  const int q0 = qb + warp * 16;
+  const float* Qw = Qs + warp * 16 * LDS;
+  const float c = scale * kLog2e;
+
+  float o[DH / 8][4];
+#pragma unroll
+  for (int i = 0; i < DH / 8; ++i) { o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f; }
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+
+  // the mask and tile skipping of attn_fwd_kernel (cond >= 0 always here)
+  const int lim0 = max(q0 + g, cond - 1), lim1 = max(q0 + g + 8, cond - 1);
+  const int ntiles = min((N + KB - 1) / KB, max(min(N - 1, qb + kWideRows - 1), cond - 1) / KB + 1);
+  load_tile<DH, kWideRows, 256>(Qs, qbase, ld, qb, N, tid);
+  load_tile<DH, KB, 256>(Ks, kbase, ld, 0, N, tid);
+  load_tile<DH, KB, 256>(Vs, vbase, ld, 0, N, tid);
+  cpa_commit();
+  for (int j = 0; j < ntiles; ++j) {
+    const int buf = j & 1;
+    cpa_wait<0>();
+    __syncthreads();
+    if (j + 1 < ntiles) {
+      load_tile<DH, KB, 256>(Ks + (buf ^ 1) * TILE, kbase, ld, (j + 1) * KB, N, tid);
+      load_tile<DH, KB, 256>(Vs + (buf ^ 1) * TILE, vbase, ld, (j + 1) * KB, N, tid);
+      cpa_commit();
+    }
+    float s[NT][4];
+#pragma unroll
+    for (int i = 0; i < NT; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
+    mma_srows_x_tileT<DH, PASSES, NT>(s, Qw, Ks + buf * TILE, lane);
+    if ((j + 1) * KB > N || j * KB + KB - 1 > min(lim0, lim1)) {
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt) {
+        const int key = j * KB + nt * 8 + 2 * t;
+        if (key >= N || key > lim0) s[nt][0] = -INFINITY;
+        if (key + 1 >= N || key + 1 > lim0) s[nt][1] = -INFINITY;
+        if (key >= N || key > lim1) s[nt][2] = -INFINITY;
+        if (key + 1 >= N || key + 1 > lim1) s[nt][3] = -INFINITY;
+      }
+    }
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      mx0 = fmaxf(mx0, fmaxf(s[nt][0], s[nt][1]));
+      mx1 = fmaxf(mx1, fmaxf(s[nt][2], s[nt][3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+    const float al0 = exp2f((m0 - mn0) * c), al1 = exp2f((m1 - mn1) * c);
+    m0 = mn0; m1 = mn1;
+    l0 *= al0; l1 *= al1;
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) { o[i][0] *= al0; o[i][1] *= al0; o[i][2] *= al1; o[i][3] *= al1; }
+    uint32_t pf[NT][4];
+    const float mc0 = m0 * c, mc1 = m1 * c;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      const float p0 = exp2f(s[nt][0] * c - mc0), p1 = exp2f(s[nt][1] * c - mc0);
+      const float p2 = exp2f(s[nt][2] * c - mc1), p3 = exp2f(s[nt][3] * c - mc1);
+      l0 += p0 + p1; l1 += p2 + p3;
+      acc_to_a<PASSES>(pf[nt], p0, p1, p2, p3);
+    }
+    mma_pn_x_tile<DH, PASSES, NT>(o, pf, Vs + buf * TILE, lane);
+  }
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+  const int r0 = q0 + g, r1 = q0 + g + 8;
+  const long long ob = (long long)b * N * inner + h * DH;
+#pragma unroll
+  for (int dt = 0; dt < DH / 8; ++dt) {
+    if (r0 < N) store2<0>(out, ob + (long long)r0 * inner + dt * 8 + 2 * t, o[dt][0] * inv0, o[dt][1] * inv0, round_out);
+    if (r1 < N) store2<0>(out, ob + (long long)r1 * inner + dt * 8 + 2 * t, o[dt][2] * inv1, o[dt][3] * inv1, round_out);
+  }
+  if (t == 0) {
+    float* lb = lse + ((long long)b * heads + h) * N;
+    if (r0 < N) lb[r0] = m0 * scale + logf(l0);
+    if (r1 < N) lb[r1] = m1 * scale + logf(l1);
+  }
+}
+
+// backward, key side: grid (ceil(N/128), heads, B); K[128 rows], V[128 rows], Q[2][32 rows], dO[2][32 rows], lse[2][32],
+// delta[2][32].  Transposed score tiles as in attn_bwd_dkv_kernel.
+template <int DH, int PASSES>
+__global__ void __launch_bounds__(256, 1)
+attn_bwd_dkv_wide_kernel(const float* __restrict__ qkv, const float* __restrict__ dout, const float* __restrict__ lse,
+                         const float* __restrict__ delta, float* __restrict__ dqkv, int N, int heads, float scale, int cond,
+                         int round_out) {
+  constexpr int LDS = Pitch<float, DH>::LDS;
+  constexpr int KB = 32, NT = KB / 8;
+  constexpr int TILE = KB * LDS;
+  extern __shared__ __align__(16) uint8_t sm_raw[];
+  float* Kr = reinterpret_cast<float*>(sm_raw);
+  float* Vr = Kr + kWideRows * LDS;
+  float* Qs = Vr + kWideRows * LDS;
+  float* Ds = Qs + 2 * TILE;
+  float* Ls = Ds + 2 * TILE;
+  float* Es = Ls + 2 * KB;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int inner = heads * DH;
+  const long long ld = 3ll * inner;
+  const float* qbase = qkv + (long long)b * N * ld + h * DH;
+  const float* dobase = dout + (long long)b * N * inner + h * DH;
+  const float* lb = lse + ((long long)b * heads + h) * N;
+  const float* eb = delta + ((long long)b * heads + h) * N;
+  const int kb = blockIdx.x * kWideRows;
+  const int k0 = kb + warp * 16;
+  const float* Kw = Kr + warp * 16 * LDS;
+  const float* Vw = Vr + warp * 16 * LDS;
+  const float c = scale * kLog2e;
+
+  float dk[DH / 8][4], dv[DH / 8][4];
+#pragma unroll
+  for (int i = 0; i < DH / 8; ++i) { dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.f; dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f; }
+
+  auto stage = [&](int j, int buf) {
+    load_tile<DH, KB, 256>(Qs + buf * TILE, qbase, ld, j * KB, N, tid);
+    load_tile<DH, KB, 256>(Ds + buf * TILE, dobase, inner, j * KB, N, tid);
+    if (tid < KB) {
+      const int q = j * KB + tid;
+      Ls[buf * KB + tid] = q < N ? lb[q] * kLog2e : INFINITY;   // +inf -> P = 0 for padded queries
+      Es[buf * KB + tid] = q < N ? eb[q] : 0.f;
+    }
+  };
+  const int ntiles = (N + KB - 1) / KB;
+  // key k receives from query q iff k <= max(q, cond - 1): a CTA whose first key is at or past `cond` starts at its own
+  // first key's query tile
+  const int jbeg = kb >= cond ? kb / KB : 0;
+  const int kr0 = k0 + g, kr1 = k0 + g + 8;
+  load_tile<DH, kWideRows, 256>(Kr, qbase + inner, ld, kb, N, tid);
+  load_tile<DH, kWideRows, 256>(Vr, qbase + 2 * inner, ld, kb, N, tid);
+  stage(jbeg, 0);
+  cpa_commit();
+  for (int j = jbeg; j < ntiles; ++j) {
+    const int buf = (j - jbeg) & 1;
+    cpa_wait<0>();
+    __syncthreads();
+    if (j + 1 < ntiles) { stage(j + 1, buf ^ 1); cpa_commit(); }
+    const float* Q = Qs + buf * TILE;
+    const float* dO = Ds + buf * TILE;
+    float s[NT][4];
+#pragma unroll
+    for (int i = 0; i < NT; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
+    mma_srows_x_tileT<DH, PASSES, NT>(s, Kw, Q, lane);       // S^T = K Q^T
+    uint32_t pf[NT][4];
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      const float la = Ls[buf * KB + nt * 8 + 2 * t], lbb = Ls[buf * KB + nt * 8 + 2 * t + 1];
+      s[nt][0] = exp2f(s[nt][0] * c - la);  s[nt][1] = exp2f(s[nt][1] * c - lbb);
+      s[nt][2] = exp2f(s[nt][2] * c - la);  s[nt][3] = exp2f(s[nt][3] * c - lbb);
+      const int va = max(j * KB + nt * 8 + 2 * t, cond - 1), vb = max(j * KB + nt * 8 + 2 * t + 1, cond - 1);   // last key each query sees
+      if (kr0 > va) s[nt][0] = 0.f;
+      if (kr0 > vb) s[nt][1] = 0.f;
+      if (kr1 > va) s[nt][2] = 0.f;
+      if (kr1 > vb) s[nt][3] = 0.f;
+      acc_to_a<PASSES>(pf[nt], s[nt][0], s[nt][1], s[nt][2], s[nt][3]);
+    }
+    mma_pn_x_tile<DH, PASSES, NT>(dv, pf, dO, lane);         // dV += P^T dO
+    float dp[NT][4];
+#pragma unroll
+    for (int i = 0; i < NT; ++i) { dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f; }
+    mma_srows_x_tileT<DH, PASSES, NT>(dp, Vw, dO, lane);     // dP^T = V dO^T
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      const float ea = Es[buf * KB + nt * 8 + 2 * t], ebb = Es[buf * KB + nt * 8 + 2 * t + 1];
+      acc_to_a<PASSES>(pf[nt], s[nt][0] * (dp[nt][0] - ea), s[nt][1] * (dp[nt][1] - ebb), s[nt][2] * (dp[nt][2] - ea),
+                       s[nt][3] * (dp[nt][3] - ebb));
+    }
+    mma_pn_x_tile<DH, PASSES, NT>(dk, pf, Q, lane);          // dK += dS^T Q
+  }
+  const long long dkb = (long long)b * N * ld + inner + h * DH;
+  const long long dvb = dkb + inner;
+#pragma unroll
+  for (int dt = 0; dt < DH / 8; ++dt) {
+    if (kr0 < N) {
+      store2<0>(dqkv, dkb + (long long)kr0 * ld + dt * 8 + 2 * t, dk[dt][0] * scale, dk[dt][1] * scale, round_out);
+      store2<0>(dqkv, dvb + (long long)kr0 * ld + dt * 8 + 2 * t, dv[dt][0], dv[dt][1], round_out);
+    }
+    if (kr1 < N) {
+      store2<0>(dqkv, dkb + (long long)kr1 * ld + dt * 8 + 2 * t, dk[dt][2] * scale, dk[dt][3] * scale, round_out);
+      store2<0>(dqkv, dvb + (long long)kr1 * ld + dt * 8 + 2 * t, dv[dt][2], dv[dt][3], round_out);
+    }
+  }
+}
+
+// backward, query side: grid (ceil(N/128), heads, B); Q[128 rows], dO[128 rows], K[2][32 rows], V[2][32 rows]
+template <int DH, int PASSES>
+__global__ void __launch_bounds__(256, 1)
+attn_bwd_dq_wide_kernel(const float* __restrict__ qkv, const float* __restrict__ dout, const float* __restrict__ lse,
+                        const float* __restrict__ delta, float* __restrict__ dqkv, int N, int heads, float scale, int cond,
+                        int round_out) {
+  constexpr int LDS = Pitch<float, DH>::LDS;
+  constexpr int KB = 32, NT = KB / 8;
+  constexpr int TILE = KB * LDS;
+  extern __shared__ __align__(16) uint8_t sm_raw[];
+  float* Qr = reinterpret_cast<float*>(sm_raw);
+  float* Dr = Qr + kWideRows * LDS;
+  float* Ks = Dr + kWideRows * LDS;
+  float* Vs = Ks + 2 * TILE;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int inner = heads * DH;
+  const long long ld = 3ll * inner;
+  const float* qbase = qkv + (long long)b * N * ld + h * DH;
+  const float* kbase = qbase + inner;
+  const float* vbase = qbase + 2 * inner;
+  const float* dobase = dout + (long long)b * N * inner + h * DH;
+  const int qb = blockIdx.x * kWideRows;
+  const int q0 = qb + warp * 16;
+  const float* Qw = Qr + warp * 16 * LDS;
+  const float* Dw = Dr + warp * 16 * LDS;
+  const float c = scale * kLog2e;
+  const int r0 = q0 + g, r1 = q0 + g + 8;
+  const float* lb = lse + ((long long)b * heads + h) * N;
+  const float* eb = delta + ((long long)b * heads + h) * N;
+  const float lse0 = r0 < N ? lb[r0] * kLog2e : INFINITY, lse1 = r1 < N ? lb[r1] * kLog2e : INFINITY;
+  const float e0 = r0 < N ? eb[r0] : 0.f, e1 = r1 < N ? eb[r1] : 0.f;
+
+  float dq[DH / 8][4];
+#pragma unroll
+  for (int i = 0; i < DH / 8; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
+
+  const int lim0 = max(r0, cond - 1), lim1 = max(r1, cond - 1);
+  const int ntiles = min((N + KB - 1) / KB, max(min(N - 1, qb + kWideRows - 1), cond - 1) / KB + 1);
+  load_tile<DH, kWideRows, 256>(Qr, qbase, ld, qb, N, tid);
+  load_tile<DH, kWideRows, 256>(Dr, dobase, inner, qb, N, tid);
+  load_tile<DH, KB, 256>(Ks, kbase, ld, 0, N, tid);
+  load_tile<DH, KB, 256>(Vs, vbase, ld, 0, N, tid);
+  cpa_commit();
+  for (int j = 0; j < ntiles; ++j) {
+    const int buf = j & 1;
+    cpa_wait<0>();
+    __syncthreads();
+    if (j + 1 < ntiles) {
+      load_tile<DH, KB, 256>(Ks + (buf ^ 1) * TILE, kbase, ld, (j + 1) * KB, N, tid);
+      load_tile<DH, KB, 256>(Vs + (buf ^ 1) * TILE, vbase, ld, (j + 1) * KB, N, tid);
+      cpa_commit();
+    }
+    float s[NT][4], dp[NT][4];
+#pragma unroll
+    for (int i = 0; i < NT; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f; }
+    mma_srows_x_tileT<DH, PASSES, NT>(s, Qw, Ks + buf * TILE, lane);    // S = Q K^T
+    mma_srows_x_tileT<DH, PASSES, NT>(dp, Dw, Vs + buf * TILE, lane);   // dP = dO V^T
+    uint32_t pf[NT][4];
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      const int key = j * KB + nt * 8 + 2 * t;
+      const bool ka = key < N, kbv = key + 1 < N;
+      const float p0 = (ka && key <= lim0) ? exp2f(s[nt][0] * c - lse0) : 0.f, p1 = (kbv && key + 1 <= lim0) ? exp2f(s[nt][1] * c - lse0) : 0.f;
+      const float p2 = (ka && key <= lim1) ? exp2f(s[nt][2] * c - lse1) : 0.f, p3 = (kbv && key + 1 <= lim1) ? exp2f(s[nt][3] * c - lse1) : 0.f;
+      acc_to_a<PASSES>(pf[nt], p0 * (dp[nt][0] - e0), p1 * (dp[nt][1] - e0), p2 * (dp[nt][2] - e1), p3 * (dp[nt][3] - e1));
+    }
+    mma_pn_x_tile<DH, PASSES, NT>(dq, pf, Ks + buf * TILE, lane);       // dQ += dS K
+  }
+  const long long dqb = (long long)b * N * ld + h * DH;
+#pragma unroll
+  for (int dt = 0; dt < DH / 8; ++dt) {
+    if (r0 < N) store2<0>(dqkv, dqb + (long long)r0 * ld + dt * 8 + 2 * t, dq[dt][0] * scale, dq[dt][1] * scale, round_out);
+    if (r1 < N) store2<0>(dqkv, dqb + (long long)r1 * ld + dt * 8 + 2 * t, dq[dt][2] * scale, dq[dt][3] * scale, round_out);
+  }
+}
+
+template <int DH, int PASSES>
+static int fwd_wide_launch(const float* qkv, float* out, float* lse, int B, int N, int heads, float scale, int cond, int round_out,
+                           cudaStream_t s) {
+  constexpr size_t smem = (kWideRows + 4 * 64) * Pitch<float, DH>::LDS * sizeof(float);
+  auto kern = attn_fwd_wide_kernel<DH, PASSES>;
+  B200_CONFIGURE_SMEM_ONCE(kern, smem);
+  kern<<<dim3((N + kWideRows - 1) / kWideRows, heads, B), 256, smem, s>>>(qkv, out, lse, N, heads, scale, cond, round_out);
+  B200_LAUNCH_OK("attn_fwd_wide_kernel");
+  return 0;
+}
+
+template <int DH, int PASSES>
+static int bwd_wide_launch(const float* qkv, const float* dout, const float* lse, const float* delta, float* dqkv, int B, int N,
+                           int heads, float scale, int cond, int round_out, cudaStream_t s) {
+  constexpr size_t rows = 2 * kWideRows + 4 * 32;
+  constexpr size_t smem_kv = rows * Pitch<float, DH>::LDS * sizeof(float) + 4 * 32 * sizeof(float);
+  constexpr size_t smem_q = rows * Pitch<float, DH>::LDS * sizeof(float);
+  auto k1 = attn_bwd_dkv_wide_kernel<DH, PASSES>;
+  auto k2 = attn_bwd_dq_wide_kernel<DH, PASSES>;
+  B200_CONFIGURE_SMEM_ONCE(k1, smem_kv);
+  B200_CONFIGURE_SMEM_ONCE(k2, smem_q);
+  const dim3 grid((N + kWideRows - 1) / kWideRows, heads, B);
+  k1<<<grid, 256, smem_kv, s>>>(qkv, dout, lse, delta, dqkv, N, heads, scale, cond, round_out);
+  B200_LAUNCH_OK("attn_bwd_dkv_wide_kernel");
+  k2<<<grid, 256, smem_q, s>>>(qkv, dout, lse, delta, dqkv, N, heads, scale, cond, round_out);
+  B200_LAUNCH_OK("attn_bwd_dq_wide_kernel");
+  return 0;
+}
+
+static int check_wide(const void* qkv, int B, int N, int heads, int dh, int cond_len) {
+  B200_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attention: empty problem");
+  B200_CHECK_ARG(dh == 96 || dh == 128, "attention: wide-head core takes head size 96 or 128 (got %d)", dh);
+  B200_CHECK_ARG(B <= 65535 && heads <= 65535, "attention: grid too large");
+  B200_CHECK_ARG(cond_len >= 0 && cond_len <= N, "attention: cond_len %d outside [0, %d]", cond_len, N);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0, "attention: qkv must be 16-byte aligned");
+  return 0;
+}
+
+int attention_wide_forward(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale, int cond_len,
+                           int exact, int round_out, cudaStream_t stream) {
+  if (int rc = check_wide(qkv, B, N, heads, dh, cond_len)) return rc;
+  if (exact) return dh == 128 ? fwd_wide_launch<128, 3>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream)
+                              : fwd_wide_launch<96, 3>(qkv, out, lse, B, N, heads, scale, cond_len, 0, stream);
+  return dh == 128 ? fwd_wide_launch<128, 1>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream)
+                   : fwd_wide_launch<96, 1>(qkv, out, lse, B, N, heads, scale, cond_len, round_out, stream);
+}
+
+int attention_wide_backward(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv, float* delta,
+                            int B, int N, int heads, int dh, float scale, int cond_len, int exact, int round_out,
+                            cudaStream_t stream) {
+  if (int rc = check_wide(qkv, B, N, heads, dh, cond_len)) return rc;
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(dout) & 15) == 0, "attention: dout must be 16-byte aligned");
+  if (int rc = attention_delta(out, 0, dout, 0, delta, B, N, heads, dh, stream)) return rc;
+  if (exact) return dh == 128 ? bwd_wide_launch<128, 3>(qkv, dout, lse, delta, dqkv, B, N, heads, scale, cond_len, 0, stream)
+                              : bwd_wide_launch<96, 3>(qkv, dout, lse, delta, dqkv, B, N, heads, scale, cond_len, 0, stream);
+  return dh == 128 ? bwd_wide_launch<128, 1>(qkv, dout, lse, delta, dqkv, B, N, heads, scale, cond_len, round_out, stream)
+                   : bwd_wide_launch<96, 1>(qkv, dout, lse, delta, dqkv, B, N, heads, scale, cond_len, round_out, stream);
+}
 
 // ---------------------------------------------------------------------------------------------
 template <int DH, int PASSES, int OUT16>

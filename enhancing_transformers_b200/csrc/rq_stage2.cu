@@ -369,7 +369,7 @@ static int short_check(const void* a, const void* b, const void* c, long long ns
   B200_CHECK_ARG(a && b && c, "%s: null pointer argument", what);
   B200_CHECK_ARG(nseq > 0 && heads > 0, "%s: bad shape (sequences=%lld heads=%d)", what, nseq, heads);
   B200_CHECK_ARG(D >= 1 && D <= kShortMaxD, "%s: sequence length must be 1..%d (got %d)", what, kShortMaxD, D);
-  B200_CHECK_ARG(hs == 32 || hs == 64, "%s: head size must be 32 or 64 (got %d)", what, hs);
+  B200_CHECK_ARG(hs == 32 || hs == 64 || hs == 96 || hs == 128, "%s: head size must be 32, 64, 96 or 128 (got %d)", what, hs);
   B200_CHECK_ARG(heads * hs <= 2048, "%s: heads * head size must be <= 2048 (got %d)", what, heads * hs);
   B200_CHECK_ARG(cond >= 0, "%s: cond_len must be >= 0 (got %d)", what, cond);
   B200_CHECK_ARG(nseq * heads < (1LL << 31), "%s: too many (sequence, head) pairs", what);
@@ -390,10 +390,43 @@ static int short_warps(size_t warp_bytes) {
   return w < 1 ? 1 : (w > 8 ? 8 : w);
 }
 
+// Head sizes 96 / 128: a warp's staged rows take up to 27 KB (forward) / 36 KB (backward) at D = 16, so the CTA's rows are
+// sized against a larger opt-in budget, which still lets two CTAs share an SM.
+constexpr size_t kShortWideSmem = 110 * 1024;
+static int short_warps_wide(size_t warp_bytes) {
+  const int w = (int)(kShortWideSmem / warp_bytes);
+  return w > 8 ? 8 : w;                                   // >= 3: warp_bytes <= 36 KB for D <= 16
+}
+
+template <int HS>
+static int short_fwd_wide(const float* qkv, float* out, long long nseq, int D, int heads, int cond, float scale, cudaStream_t stream) {
+  const size_t wb = short_warp_floats(D, HS, 3) * sizeof(float);
+  const int wpb = short_warps_wide(wb);
+  auto kern = short_attention_fwd_kernel<HS>;
+  B200_CONFIGURE_SMEM_ONCE(kern, kShortWideSmem);
+  kern<<<short_grid(nseq * heads, wpb), wpb * 32, wpb * wb, stream>>>(qkv, out, nseq, D, heads, cond, scale);
+  B200_LAUNCH_OK("short_attention_fwd_kernel");
+  return 0;
+}
+
+template <int HS>
+static int short_bwd_wide(const float* qkv, const float* dout, float* dqkv, long long nseq, int D, int heads, int cond, float scale,
+                          cudaStream_t stream) {
+  const size_t wb = short_warp_floats(D, HS, 4) * sizeof(float);
+  const int wpb = short_warps_wide(wb);
+  auto kern = short_attention_bwd_kernel<HS>;
+  B200_CONFIGURE_SMEM_ONCE(kern, kShortWideSmem);
+  kern<<<short_grid(nseq * heads, wpb), wpb * 32, wpb * wb, stream>>>(qkv, dout, dqkv, nseq, D, heads, cond, scale);
+  B200_LAUNCH_OK("short_attention_bwd_kernel");
+  return 0;
+}
+
 extern "C" int b200vq_short_attention_fwd(const float* qkv, float* out, long long nseq, int D, int heads, int hs, int cond,
                                           float scale, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = short_check(qkv, out, out, nseq, D, heads, hs, cond, "short_attention_fwd")) return rc;
+  if (hs == 128) return short_fwd_wide<128>(qkv, out, nseq, D, heads, cond, scale, stream);
+  if (hs == 96) return short_fwd_wide<96>(qkv, out, nseq, D, heads, cond, scale, stream);
   const size_t wb = short_warp_floats(D, hs, 3) * sizeof(float);
   const int wpb = short_warps(wb);
   const int grid = short_grid(nseq * heads, wpb);
@@ -407,6 +440,8 @@ extern "C" int b200vq_short_attention_bwd(const float* qkv, const float* dout, f
                                           int cond, float scale, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
   if (int rc = short_check(qkv, dout, dqkv, nseq, D, heads, hs, cond, "short_attention_bwd")) return rc;
+  if (hs == 128) return short_bwd_wide<128>(qkv, dout, dqkv, nseq, D, heads, cond, scale, stream);
+  if (hs == 96) return short_bwd_wide<96>(qkv, dout, dqkv, nseq, D, heads, cond, scale, stream);
   const size_t wb = short_warp_floats(D, hs, 4) * sizeof(float);
   const int wpb = short_warps(wb);
   const int grid = short_grid(nseq * heads, wpb);

@@ -184,7 +184,8 @@ copy_rows_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, 
 
 // Sampling step (layers.py:66-81 with use_cache and layer_past): block (h, b) appends this step's key / value rows of its head
 // to the cache at position `pos`, then attends its single query to cache rows 0 .. pos (no mask):
-// scores -> shared memory, block-wide max / sum, out[d] = sum_j p_j V[j, d] with one thread per head dim.
+// scores -> shared memory, block-wide max / sum, out[d] = sum_j p_j V[j, d] with one thread per head dim (HS <= 128 = the
+// block size).
 // qkv [B, 3*C] (q | k | v thirds), cache_k / cache_v [B, Tmax, C], out [B, C].
 template <int HS>
 __global__ void __launch_bounds__(128)
@@ -347,14 +348,17 @@ extern "C" int b200vq_copy_rows(const float* src, float* dst, int B, int T_src, 
 extern "C" int b200vq_decode_attention(const float* qkv, float* cache_k, float* cache_v, float* out, int B, int heads, int hs,
                                        int Tmax, int pos, float scale, void* streamv) {
   const cudaStream_t stream = static_cast<cudaStream_t>(streamv);
-  B200_CHECK_ARG(B > 0 && heads > 0 && (hs == 32 || hs == 64), "decode_attention: head size must be 32 or 64 (got %d)", hs);
+  B200_CHECK_ARG(B > 0 && heads > 0 && (hs == 32 || hs == 64 || hs == 96 || hs == 128),
+                 "decode_attention: head size must be 32, 64, 96 or 128 (got %d)", hs);
   B200_CHECK_ARG(pos >= 0 && pos < Tmax, "decode_attention: position %d outside the cache (%d rows)", pos, Tmax);
   B200_CHECK_ARG(B <= 65535, "decode_attention: batch too large");
   const int C = heads * hs;
   const size_t smem = (size_t)(pos + 1) * sizeof(float);
   B200_CHECK_ARG(smem <= 40 * 1024, "decode_attention: context of %d keys exceeds the score buffer", pos + 1);
-  if (hs == 64) decode_attention_kernel<64><<<dim3(heads, B), 128, smem, stream>>>(qkv, cache_k, cache_v, out, C, Tmax, pos, scale);
-  else          decode_attention_kernel<32><<<dim3(heads, B), 128, smem, stream>>>(qkv, cache_k, cache_v, out, C, Tmax, pos, scale);
+  if (hs == 128)     decode_attention_kernel<128><<<dim3(heads, B), 128, smem, stream>>>(qkv, cache_k, cache_v, out, C, Tmax, pos, scale);
+  else if (hs == 96) decode_attention_kernel<96><<<dim3(heads, B), 128, smem, stream>>>(qkv, cache_k, cache_v, out, C, Tmax, pos, scale);
+  else if (hs == 64) decode_attention_kernel<64><<<dim3(heads, B), 128, smem, stream>>>(qkv, cache_k, cache_v, out, C, Tmax, pos, scale);
+  else               decode_attention_kernel<32><<<dim3(heads, B), 128, smem, stream>>>(qkv, cache_k, cache_v, out, C, Tmax, pos, scale);
   B200_LAUNCH_OK("decode_attention_kernel");
   return 0;
 }

@@ -12,8 +12,10 @@ HBM streams (csrc/stage2.cu).
 Data path (``etb.set_precision``): "fp16" (default) -> the Linear layers on f16 GEMMs (fp16 operands, fp32 accumulate and
 output, per-call power-of-two gradient scaling chosen on the device), attention core on tf32; "tf32" -> everything
 tf32; "parity" -> 3xTF32 GEMMs and attention (fp32-grade).  Limits of the kernels underneath, raised at construction:
-head size ``embed_dim // n_heads`` must be 32 or 64, ``embed_dim`` <= 2048, ``vocab_img_size`` % 64 == 0 (the YAML's 6144 / 16 = 384-wide heads --
-a 10.9 B-parameter model that cannot train under replicated fp32 DDP anyway, SURVEY.md section 8f-3 -- are not covered).
+head size ``embed_dim // n_heads`` must be 32, 64, 96 or 128, ``embed_dim`` <= 2048 and a multiple of 64, ``vocab_img_size`` % 64 == 0
+(the YAML's 6144 / 16 = 384-wide heads -- a 10.9 B-parameter model that cannot train under replicated fp32 DDP anyway, SURVEY.md
+section 8f-3 -- are not covered).  Heads of 96 and 128 run on wide-head kernels that keep their resident operands in shared
+memory (DESIGN.md section 4.2); 32 and 64 on the register-resident ones.
 
 ``RQTransformer`` (reference :306-547, the prior over residual codes [B, T, D]) reuses these blocks: its spatial transformer is
 ``GPT``'s, its depth transformer runs causal attention over B*T sequences of D <= 16 tokens on the short-sequence kernel of
@@ -269,11 +271,14 @@ class RQDepthInputFn(torch.autograd.Function):
         return gh, None, gWi, gpd.view(shape_d)
 
 
+HEAD_SIZES = (32, 64, 96, 128)    # head sizes the attention, KV-cache and depth kernels take
+
+
 def _check_kernel_limits(embed_dim: int, n_heads: int) -> None:
     assert embed_dim % n_heads == 0
     hs = embed_dim // n_heads
-    if hs not in (32, 64):
-        raise NotImplementedError(f"b200vq stage 2: head size embed_dim // n_heads must be 32 or 64 (got {hs}); "
+    if hs not in HEAD_SIZES:
+        raise NotImplementedError(f"b200vq stage 2: head size embed_dim // n_heads must be 32, 64, 96 or 128 (got {hs}); "
                                   "use the reference modules for this geometry")
     if embed_dim > 2048 or embed_dim % 64:
         raise NotImplementedError(f"b200vq stage 2: embed_dim must be a multiple of 64 and <= 2048 (got {embed_dim})")
@@ -540,8 +545,8 @@ class RQTransformer(nn.Module):
     residual codes of each position.  Reproduces what the reference computes, quirks included: the code embeddings are
     prefix sums over the channel axis (`cumsum(-1)`, :378), the sampler embeds codes as sums over depth (:502, :535) and
     applies `ln_depth` twice on depth step 0 (:531, :542).  Limits of the kernels underneath, raised at construction: head
-    sizes 32 / 64 (spatial and depth), `embed_dim` <= 2048 and a multiple of 64, `vocab_img_size` % 64 == 0,
-    2 <= `depth_num_tokens` <= 16."""
+    sizes 32 / 64 / 96 / 128 (spatial and depth, chosen independently), `embed_dim` <= 2048 and a multiple of 64,
+    `vocab_img_size` % 64 == 0, 2 <= `depth_num_tokens` <= 16."""
 
     def __init__(self, vocab_cond_size: int, vocab_img_size: int, embed_dim: int, cond_num_tokens: int, img_num_tokens: int,
                  depth_num_tokens: int, spatial_n_heads: int, depth_n_heads: int, spatial_n_layers: int, depth_n_layers: int,

@@ -219,7 +219,9 @@ int b200vq_upfirdn2d(const float* in, const float* kernel, float* out, long long
  *   mask of layers.py:43-48,83-85: query q attends to key k iff k <= max(q, cond_len - 1) -- causal, the cond_len
  *   condition tokens fully visible to each other.  exact != 0: error-compensated 3xTF32 (precision="parity");
  *   otherwise the single-pass tf32 kernels (round_out as in b200vq_attention_fwd).  dh (the head size
- *   embed_dim / n_heads) must be 32 or 64.
+ *   embed_dim / n_heads) must be 32, 64, 96 or 128; 96 and 128 run on wide-head kernels that read their resident operand
+ *   from shared memory, with the same mask, LSE, round_out and bit-reproducibility (no atomics).  The stage-1 entry
+ *   points above keep their head sizes.
  * time_mix: y = x * w + shift(x) * (1 - w), shift = one step along T with a zero first row (layers.py:50-58), bit-identical
  *   to the reference's four fp32 tensor ops.  x, y [M = B*T, C]; w [C].
  *   bwd: gx likewise; gw_part [ceil(M / 64), C] holds per-64-row partial sums of g * (x - shift(x)) -- b200vq_colsum over
@@ -234,7 +236,7 @@ int b200vq_upfirdn2d(const float* in, const float* kernel, float* out, long long
  *   x[:, cond-1:-1] of layers.py:210 and its zero-padded gradient).
  * decode_attention: one sampling step of layers.py:66-81 (use_cache with layer_past): appends the k / v thirds of
  *   qkv [B, 3*C] to cache_k / cache_v [B, Tmax, C] at row `pos` and writes softmax(q K^T * scale) V over rows 0..pos
- *   to out [B, C]. */
+ *   to out [B, C].  hs 32, 64, 96 or 128. */
 int b200vq_attention_causal_fwd(const float* qkv, float* out, float* lse, int B, int N, int heads, int dh, float scale,
                                 int cond_len, int exact, int round_out, void* stream);
 int b200vq_attention_causal_bwd(const float* qkv, const float* out, const float* lse, const float* dout, float* dqkv,
@@ -261,7 +263,7 @@ int b200vq_decode_attention(const float* qkv, float* cache_k, float* cache_v, fl
 /* ---- stage-2 RQTransformer (reference enhancing/modules/stage2/layers.py:306-547) ---------------------------------------
  * short_attention: the depth transformer's attention core -- nseq independent sequences of D tokens (1 <= D <= 16), the
  *   packed qkv [nseq*D, 3*heads*hs] of b200vq_attention_causal_fwd (q | k | v thirds, head h at columns h*hs) -> out
- *   [nseq*D, heads*hs]; the mask of b200vq_attention_causal_fwd (k <= max(q, cond_len - 1)); hs 32 or 64, heads*hs <= 2048.
+ *   [nseq*D, heads*hs]; the mask of b200vq_attention_causal_fwd (k <= max(q, cond_len - 1)); hs 32, 64, 96 or 128, heads*hs <= 2048.
  *   fp32 FMA arithmetic and an fp32 softmax on every data path.  bwd recomputes the scores from qkv and writes every
  *   element of dqkv [nseq*D, 3*heads*hs] (no lse / out / delta needed, no atomics: the same bits on every run).  Both
  *   are persistent grid-stride kernels: b200vq_set_sm_limit caps their grid at that many CTAs (the results do not
